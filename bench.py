@@ -39,7 +39,7 @@ METRIC = "filtered-scan Mrows/s (URL LIKE '%google%' + get-with-selection, hot c
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=100)  # a step is ~0.5 ms: 100 keep one host hiccup from deciding the mean
+    ap.add_argument("--steps", type=int, default=100)  # a step is well under a millisecond: 100 keep one host hiccup from deciding the mean
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--rows", type=int, default=100_000_000, help="rows PER GPU (weak scaling)")
@@ -54,21 +54,44 @@ def parse_args():
                     help="url_like = BASELINE configs[1] (the bench line the driver records); int_filter = configs[2]; "
                          "shipdate = configs[3] (TPC-H SF100 l_shipdate range, one GPU's shard of the 8-way split per rank); "
                          "clickbench_sweep = configs[4] (scan stage of the 43 ClickBench queries, bench_sweep.py)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="url_like: after the timed steps, write the filtered URLs the last step delivered as DIR/*.npy "
+                         "(float32 / float64, at most 64 MB; a fixed seeded sample of the rows above that)")
+    args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "url_like" or args.impl != "ours"):
+        ap.error("--dump-outputs writes the result of the url_like workload of --impl ours")
+    return args
 
 
-def recorded_traffic(rows: int, entries: int):
-    """DRAM bytes (read + write) of one k_str_like launch, REPLAYED from the committed `ncu --set full` capture of this
-    exact seeded workload (profiles/r02_k_str_like_traffic.json) — not measured in this run; None when the shape differs
-    or the file is absent. A number taken under the profiler is only ever used for this field, never for a timing."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_k_str_like_traffic.json")) as f:
-            t = json.load(f)
-        if t["workload"]["rows"] == rows and t["workload"]["entries"] == entries:
-            return int(t["dram__bytes_read.sum"]) + int(t["dram__bytes_write.sum"])
-    except (OSError, KeyError, ValueError):
-        pass
-    return None
+DUMP_LIMIT = 64 << 20
+
+
+def dump_string_array(out_dir: str, name: str, arr) -> None:
+    """A host Arrow string array as DIR/<name>_offsets.npy (float64, n + 1 value offsets) and DIR/<name>_bytes.npy
+    (float32, one element per UTF-8 byte), so that two builds can be compared output for output. Above DUMP_LIMIT bytes
+    the rows of a fixed seeded sample are written instead, and their row numbers as DIR/<name>_rows.npy (float64)."""
+    import numpy as np
+    import pyarrow as pa
+
+    def parts(a):
+        a = pa.concat_arrays([a]) if a.offset else a
+        off = np.frombuffer(a.buffers()[1], dtype=np.int32, count=len(a) + 1).astype(np.int64)
+        data = np.frombuffer(a.buffers()[2], dtype=np.uint8)[off[0]:off[-1]] if len(a) else np.zeros(0, np.uint8)
+        return (off - off[0]).astype(np.float64), data.astype(np.float32)
+
+    rows = None
+    off, data = parts(arr)
+    if off.nbytes + data.nbytes > DUMP_LIMIT:
+        k = len(arr)
+        while off.nbytes + data.nbytes > DUMP_LIMIT:
+            k = max(1, int(k * 0.9 * DUMP_LIMIT / (off.nbytes + data.nbytes + 1)))
+            rows = np.sort(np.random.default_rng(0).choice(len(arr), size=k, replace=False))
+            off, data = parts(arr.take(pa.array(rows)))
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f"{name}_offsets.npy"), off)
+    np.save(os.path.join(out_dir, f"{name}_bytes.npy"), data)
+    if rows is not None:
+        np.save(os.path.join(out_dir, f"{name}_rows.npy"), rows.astype(np.float64))
 
 
 def measured_peak_gbs():
@@ -76,7 +99,7 @@ def measured_peak_gbs():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md; MEASURED_PEAKS.json absent)"
+        return 3350.0, "fallback 3.35 TB/s (H100 SXM data-sheet HBM3 bandwidth, not measured; MEASURED_PEAKS.json absent)"
 
 
 class ClockSampler:
@@ -96,8 +119,8 @@ class ClockSampler:
                                           "-lms", "20"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             threading.Thread(target=self._read, daemon=True).start()
             # the sampler must be up and running BEFORE the clock starts: nvidia-smi's start-up (NVML initialisation, its
-            # first device queries) takes driver locks that CUDA calls wait behind — with 20 steps of 0.16 ms in the timed
-            # region, one such stall (9.5 ms was measured) is three times the region
+            # first device queries) takes driver locks that CUDA calls wait behind — with 20 sub-millisecond steps in the
+            # timed region, one such stall can outlast the whole region
             t_end = time.perf_counter() + 3.0
             while not self.rows and time.perf_counter() < t_end and self.proc.poll() is None:
                 time.sleep(0.01)
@@ -498,7 +521,7 @@ def run_squeeze(args, rank, world, local_rank):
 
 def run_shipdate(args, rank, world, local_rank, emit=True):
     """BASELINE configs[3]: TPC-H SF100 lineitem `l_shipdate >= 1994-01-01 AND l_shipdate < 1995-01-01` (q6's date
-    range; Date32, W = 12), entries sharded across 8 B200: every rank holds one eighth of the 600 037 902 rows
+    range; Date32, W = 12), entries sharded across 8 GPUs: every rank holds one eighth of the 600 037 902 rows
     (weak scaling: at --gpus 8 the job is the whole table). Step = both conjuncts over every entry + get-with-selection
     of the survivors (~14 %). value: device-resident (result left in HBM); e2e: the same pipeline with the filtered
     Arrow array copied to the host every step. Secondary workload: prints its own JSON line."""
@@ -656,7 +679,7 @@ def run_shipdate(args, rank, world, local_rank, emit=True):
                        "result": "Arrow-layout buffers in HBM (lc_scan_read_async): value; host Arrow arrays (lc_scan_read): e2e",
                        "gathered_rows": int(gathered_rows), "host_syncs_per_step": 1, "gather_slot_bytes": gather.slot,
                        "slot_regrown_in_timed_steps": grows_in_timed, "numa": pin,
-                       "l2": "packed column (113 MB) + selections do not fit the L2 together with the 44 MB result; no flush",
+                       "l2": "the packed column (113 MB) alone is larger than the 50 MB L2; no flush",
                        "setup_seconds": setup_s, "result_matches_arrow": bool(ok),
                        "insert": {"Mrows_per_s": rows_local / insert_s / 1e6, "arrow_GB_per_s": rows_local * 4 / insert_s / 1e9,
                                   "note": "lc_cache_insert_many, 1024 batches of 8192 rows per call, host Arrow in (pageable), device transcode"}},
@@ -887,7 +910,7 @@ def run_url_like(args, rank, world, local_rank, emit=True, source=None, rows=Non
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     import gc
 
-    gc.disable()  # a collection inside a 0.5 ms step is a visible spike; re-enabled after the timed loops
+    gc.disable()  # a collection inside a sub-millisecond step is a visible spike; re-enabled after the timed loops
     ev0.record(stream)
     step_wall = []
     for _ in range(args.steps):
@@ -904,6 +927,8 @@ def run_url_like(args, rank, world, local_rank, emit=True, source=None, rows=Non
     grows_in_timed = gather.grows - grows_before
     # what the e2e arm below is compared with: THIS rank's own filtered batch, downloaded from the gathered slots
     local_last = gather.to_arrow([rank])
+    if args.dump_outputs and emit and rank == 0:
+        dump_string_array(args.dump_outputs, "url_like_urls", gather.to_arrow())  # the gathered result of the last step
 
     # where a step's time goes (untimed, after the measurement): device events between the three calls of a step
     ph = [[], [], [], []]
@@ -1003,7 +1028,7 @@ def run_url_like(args, rank, world, local_rank, emit=True, source=None, rows=Non
                 "untimed_steps_before_the_clock": max(3, args.warmup) + 3,  # --warmup, then 3 more once the clock sampler is up
                 "step_phases": step_phases,
                 "step_ms_rank0": {"min": min(step_wall), "median": float(np.median(step_wall)), "max": max(step_wall)}, "numa": numa_pin,
-                "l2": "inputs (liquid column) larger than the 126 MB L2, no flush needed",
+                "l2": "inputs (liquid column) larger than the 50 MB L2, no flush needed",
                 "setup_seconds": setup_s,
                 "insert": {"Mrows_per_s": rows_local / insert_s / 1e6, "arrow_GB_per_s": arrow_bytes / insert_s / 1e9,
                            "note": "lc_cache_insert_many, 256 batches of 8192 rows per call, host Arrow in, device transcode (k_str_encode.cu *_many), single stream"},
@@ -1013,8 +1038,7 @@ def run_url_like(args, rank, world, local_rank, emit=True, source=None, rows=Non
                     "matches_device_path": bool(e2e_ok)},
             "gpu_launches": launches,
             "roofline": {"bound": "hbm", "kernel": "k_str_like<MODE_REFINE>", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": recorded_traffic(rows_local, n_entries) if source == "synthetic" else None,
-                         "traffic_source": "replayed from profiles/r02_k_str_like_traffic.json (ncu --set full of this seeded workload), not measured in this run",
+                         "frac": achieved / peak,
                          "algorithmic_bytes_per_launch": algo_bytes,
                          "gate_bytes_read": gate_bytes,
                          "bytes_this_kernel_must_move": kernel_reads,

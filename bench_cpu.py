@@ -27,9 +27,8 @@ def physical_cores() -> int:
 
 def usable_cpus() -> tuple[int, dict]:
     """Threads the CPU arm should run: the logical CPUs this process may use, capped by the container's CPU quota
-    (cgroup v2 cpu.max / v1 cfs quota). Measured on the round-2 GPU box (profiles/r02_cpu_scaling_url_like.json): 128
-    logical CPUs visible, cpu.max = 16 CPUs — the port scales 15.8x on 16 threads and gets THROTTLED beyond (128 threads:
-    10x), so asking for more threads than the quota makes the baseline slower, not faster."""
+    (cgroup v2 cpu.max / v1 cfs quota). A container may see far more logical CPUs than its quota grants; threads beyond
+    the quota are throttled, so asking for more of them makes the baseline slower, not faster."""
     logical = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     quota = None
     try:
@@ -60,7 +59,7 @@ class CpuArm:
         import synth
         from oracle import c_oracle as CO
 
-        CO.lib(rebuild=True)  # -march=native: built on the machine that is timed
+        CO.lib()  # -march=native: build() runs on the machine that is timed
         self.CO = CO
         self.workload = workload
         self.threads = threads

@@ -54,7 +54,7 @@ def cpu_transcode(column: str, arrays, threads: int, target_s: float = 4.0):
     per 32 batches (a row group's column chunk, transcode.rs:16-33)."""
     from oracle import c_oracle as CO
 
-    CO.lib(rebuild=True)
+    CO.lib()
     is_str = column == "URL"
 
     def run_group(g):

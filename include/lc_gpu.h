@@ -1,10 +1,10 @@
 /*
- * lc_gpu.h — C ABI of the B200-native liquid-cache hot path.
+ * lc_gpu.h — C ABI of the H100-native liquid-cache hot path.
  *
  * This is the drop-in boundary for ONE path of XiangpengHao/liquid-cache: the
  * insert() transcode Arrow -> liquid, and get() / with_selection() /
  * eval_predicate() on liquid columns, with the liquid columns resident in HBM
- * and every array-sized loop running as a hand-written sm_100a CUDA kernel.
+ * and every array-sized loop running as a hand-written sm_90a CUDA kernel.
  *
  * The reference has no FFI seam; its seam is the Rust trait
  *   trait LiquidArray            src/core/src/liquid_array/mod.rs:82-146

@@ -1,6 +1,6 @@
 """ctypes binding of include/lc_gpu.h (liblc_gpu.so).
 
-There is no fallback: if the shared library is missing, or the process has no sm_100a device,
+There is no fallback: if the shared library is missing, or the process has no sm_90a (H100) device,
 every entry point raises. Nothing here computes on the CPU.
 """
 from __future__ import annotations

@@ -12,9 +12,9 @@
 namespace lc {
 
 // Result buffers. Small ones come from the C heap. From 1 MiB on they are PAGE-LOCKED blocks recycled through a
-// process-wide pool: a device-to-host copy into pageable memory is staged by the driver and ran at ~3 GB/s for the
-// 43 MB result of the l_shipdate scan (bench.py --workload shipdate: 16 ms per step, most of it this copy), while a
-// pinned destination takes the DMA directly. Page-locking is itself slow (~10 ms per 64 MB), hence the pool: the
+// process-wide pool: a device-to-host copy into pageable memory is staged by the driver (a multi-MB result such as the
+// 43 MB one of the l_shipdate scan then costs more than the scan), while a pinned destination takes the DMA directly.
+// Page-locking is itself slow, hence the pool: the
 // Arrow release callback hands the block back (no CUDA call), and the next result of that size class reuses it.
 // The pool outlives every context on purpose — an exported array may be released after its lc_ctx is gone.
 namespace {

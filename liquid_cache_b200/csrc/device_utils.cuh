@@ -1,4 +1,4 @@
-// device_utils.cuh — sm_100a device helpers: TMA bulk copy + mbarrier, warp scans, bit sinks.
+// device_utils.cuh — sm_90a device helpers: TMA bulk copy + mbarrier, warp scans, bit sinks.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

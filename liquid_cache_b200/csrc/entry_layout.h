@@ -121,7 +121,7 @@ static_assert(sizeof(StrHeader) == 128, "StrHeader must be 128 bytes");
 // (SubstringSearch hint): a 256-bit set per dictionary value with bit trigram_bit(b[i], b[i+1], b[i+2]) for every three
 // adjacent bytes. A value can only contain a needle if it has all of the needle's trigram bits, so values failing the test
 // are skipped WITHOUT walking their codes; values passing it are still matched exactly. Measured on the bench URL column
-// (profiles/r01_filter_rates.txt): for '%google%' the reference gate passes ~40 % of the dictionary, gate + a 64-bit bigram
+// (profiles/filter_rates.py): for '%google%' the reference gate passes ~40 % of the dictionary, gate + a 64-bit bigram
 // set 5.9 %, gate + this set 0.05 % (true matches 0.017 %). Results are identical by construction; NOT LIKE keeps the
 // reference rule "invert only if the reference gate let something through". Needles shorter than three bytes have no
 // trigram: their mask is empty and only the reference gate applies.

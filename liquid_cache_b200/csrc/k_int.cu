@@ -1,4 +1,4 @@
-// k_int.cu — frame-of-reference + FastLanes bit-packed integers on sm_100a.
+// k_int.cu — frame-of-reference + FastLanes bit-packed integers on sm_90a.
 //
 // Reference semantics restated (all under /root/reference/src/core/src/liquid_array/):
 //   encode  LiquidPrimitiveArray::from_arrow_array   primitive_array.rs:159-206
@@ -8,7 +8,7 @@
 //           LiquidPrimitiveArray::to_arrow_array     primitive_array.rs:350-368
 //   filter / try_eval_predicate                      primitive_array.rs:370-379
 //
-// Design (B200): one CTA per entry (an 8192-row batch). The CTA pulls the whole entry blob
+// Design (H100): one CTA per entry (an 8192-row batch). The CTA pulls the whole entry blob
 // (header + validity + packed chunks) into shared memory with ONE TMA bulk copy, then every lane
 // decodes "its" row straight out of the FastLanes layout (two shared loads + a funnel shift), so
 // rows come out in logical order and selection -> write-offset compaction is a warp ballot plus a
@@ -532,7 +532,7 @@ cudaError_t launch_int_scan(int mode, uint32_t n_entries, const ScanIo& io, cons
   const bool pipelined = stage != 0 && 3u * (kScanFixedSmem + 2u * stage + 1024u) <= 227u * 1024u;
   const uint32_t smem = kScanFixedSmem + (pipelined ? 2u : 1u) * stage;
   static bool attr_set = false;
-  static int n_sm = 148;
+  static int n_sm = 132;
   if (!attr_set) {
     cudaError_t e;
     e = cudaFuncSetAttribute(k_int_scan<MODE_DECODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,

@@ -8,7 +8,7 @@
 //
 // Why not the staged kernel (k_int_scan) here: on narrow columns (W = 12 .. 20: dates, EventTime, ids) an entry is only
 // 12-20 KB, and a CTA that stages it by TMA, plans, synchronises and hands each of its 8 warps ONE chunk spends most of
-// its time in the per-entry bookkeeping (ncu r02: 20 warp-instructions per 32 rows, issue 55 %, DRAM 26 %). A chunk of a
+// its time in the per-entry bookkeeping rather than on the bytes. A chunk of a
 // W-bit column is W rows of 128 bytes and every thread needs exactly W 32-bit words of it (breg_math.cuh), so a warp can
 // pull its chunk straight into registers with W coalesced loads (each instruction covers one or two whole 128-byte
 // lines: the access pattern a TMA tile would give, without the shared-memory round trip and its barriers) and run the 32
@@ -58,8 +58,7 @@ __device__ __forceinline__ uint32_t bits_group(const uint8_t* packed, uint32_t c
   const uint32_t n_words = (n + 31u) >> 5;
   uint32_t survivors = 0;
   for (uint32_t c = c0; c < c1; c += CH) {
-    // (asking the next round's lines into L2 ahead of time — one prefetch per lane — was measured and is slower: 0.047
-    // against 0.045 ms at W = 12, 0.066 against 0.062 at W = 17)
+    // (asking the next round's lines into L2 ahead of time — one prefetch per lane — is a variant not taken)
     // the packed words of the CH chunks first: nothing they need is still in flight (the header came one task ahead) ...
     uint32_t a[CH][G::SUB][G::NW];
 #pragma unroll
@@ -274,9 +273,9 @@ cudaError_t launch_int_bits(int mode, uint32_t n_entries, const ScanIo& io, cons
     if (per_sm < 1) per_sm = 1;
   }
   uint32_t grid = static_cast<uint32_t>(n_sm * per_sm);  // persistent: every resident warp loops over the tasks
-  // A task is a group of eight chunks — a whole 8192-row batch: header read and predicate planned once per batch. Measured
-  // on 100 M rows at W = 17: groups of four 0.069 ms, of eight 0.062 ms; at W = 12 (75 M rows) 0.045 ms either way, and groups
-  // of two — which spread the tasks more evenly over the resident warps — 0.053 ms. LC_INT_GROUP=2 / 4 select the others.
+  // A task is a group of eight chunks — a whole 8192-row batch: header read and predicate planned once per batch. Groups
+  // of two spread the tasks more evenly over the resident warps but plan four times as often; LC_INT_GROUP=2 / 4 select
+  // the smaller groups.
   static const uint32_t cshift_pref = [] {
     const char* e = std::getenv("LC_INT_GROUP");
     return (e && e[0] == '2') ? 1u : ((e && e[0] == '4') ? 2u : 3u);

@@ -1,4 +1,4 @@
-// k_num.cu — ALP floats and u64 decimals on top of the bit-packed integer entry (sm_100a).
+// k_num.cu — ALP floats and u64 decimals on top of the bit-packed integer entry (sm_90a).
 //
 // Reference semantics restated (all under /root/reference/src/core/src/liquid_array/):
 //   float encode   get_best_exponents + encode_arrow_array            float_array.rs:609-751
@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(1024) k_alp_patches(AlpEncIo io) {
 cudaError_t launch_alp_encode(const AlpEncIo& io, cudaStream_t s) {
   if (io.n == 0) return cudaSuccess;
   uint32_t grid = (io.n + 255u) / 256u;
-  if (grid > 1184u) grid = 1184u;  // 148 SMs x 8 resident CTAs
+  if (grid > kGridStrideCap) grid = kGridStrideCap;
   if (io.is_f64) {
     k_alp_search<double><<<alp_n_combos<double>(), 256, 0, s>>>(io);
     k_alp_encode<double><<<grid, 256, 0, s>>>(io);
@@ -467,7 +467,7 @@ cudaError_t launch_squeeze_map(void* d_vals, uint32_t n, uint32_t tbits, unsigne
                                unsigned long long limit, unsigned long long bucket_width, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   uint32_t grid = (n + 255u) / 256u;
-  if (grid > 1184u) grid = 1184u;
+  if (grid > kGridStrideCap) grid = kGridStrideCap;
   switch (tbits) {
     case 8: k_squeeze_map<uint8_t><<<grid, 256, 0, s>>>(static_cast<uint8_t*>(d_vals), n, static_cast<uint8_t>(ref), quantize, limit, bucket_width); break;
     case 16: k_squeeze_map<uint16_t><<<grid, 256, 0, s>>>(static_cast<uint16_t*>(d_vals), n, static_cast<uint16_t>(ref), quantize, limit, bucket_width); break;
@@ -507,7 +507,7 @@ cudaError_t launch_date_component(const void* d_in, uint32_t n, uint32_t in_bits
                                   int32_t* d_out, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   uint32_t grid = (n + 255u) / 256u;
-  if (grid > 1184u) grid = 1184u;
+  if (grid > kGridStrideCap) grid = kGridStrideCap;
   if (in_bits == 64) k_date_component<long long><<<grid, 256, 0, s>>>(static_cast<const long long*>(d_in), n, field, ticks_per_day, d_out);
   else k_date_component<int32_t><<<grid, 256, 0, s>>>(static_cast<const int32_t*>(d_in), n, field, 0, d_out);
   return cudaGetLastError();
@@ -517,7 +517,7 @@ cudaError_t launch_date_lossy(const int32_t* d_comp, const uint32_t* d_valid, ui
                               void* d_out, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   uint32_t grid = (n + 255u) / 256u;
-  if (grid > 1184u) grid = 1184u;
+  if (grid > kGridStrideCap) grid = kGridStrideCap;
   k_date_lossy<<<grid, 256, 0, s>>>(d_comp, d_valid, n, field, ticks_per_day, d_out);
   return cudaGetLastError();
 }
@@ -525,7 +525,7 @@ cudaError_t launch_date_lossy(const int32_t* d_comp, const uint32_t* d_valid, ui
 cudaError_t launch_widen_u32(const uint32_t* d_in, uint32_t n, unsigned long long* d_out, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   uint32_t grid = (n + 255u) / 256u;
-  if (grid > 1184u) grid = 1184u;
+  if (grid > kGridStrideCap) grid = kGridStrideCap;
   k_widen_u32<<<grid, 256, 0, s>>>(d_in, n, d_out);
   return cudaGetLastError();
 }
@@ -534,7 +534,7 @@ cudaError_t launch_narrow_u64(const unsigned long long* d_in, uint32_t n, unsign
                               cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   uint32_t grid = (n + 255u) / 256u;
-  if (grid > 1184u) grid = 1184u;
+  if (grid > kGridStrideCap) grid = kGridStrideCap;
   k_narrow_u64<<<grid, 256, 0, s>>>(d_in, n, limit, d_out, d_flag);
   return cudaGetLastError();
 }
@@ -543,7 +543,7 @@ cudaError_t launch_dec_narrow(const void* d_in, const uint32_t* d_validity, uint
                               unsigned long long* d_out, uint32_t* d_flag, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   uint32_t grid = (n + 255u) / 256u;
-  if (grid > 1184u) grid = 1184u;
+  if (grid > kGridStrideCap) grid = kGridStrideCap;
   k_dec_narrow<<<grid, 256, 0, s>>>(static_cast<const unsigned long long*>(d_in), d_validity, n, width_bytes / 8u, d_out, d_flag);
   return cudaGetLastError();
 }
@@ -552,7 +552,7 @@ cudaError_t launch_dec_widen(const unsigned long long* d_in, uint64_t n, uint32_
   if (n == 0) return cudaSuccess;
   const uint64_t total = n * (width_bytes / 8u);
   uint64_t grid = (total + 255u) / 256u;
-  if (grid > 4736u) grid = 4736u;  // 148 SMs x 8 CTAs x 4 waves
+  if (grid > 4u * kGridStrideCap) grid = 4u * kGridStrideCap;  // 4 waves
   k_dec_widen<<<static_cast<uint32_t>(grid), 256, 0, s>>>(d_in, n, width_bytes / 8u, static_cast<unsigned long long*>(d_out));
   return cudaGetLastError();
 }

@@ -51,9 +51,8 @@ __device__ __forceinline__ void block_scan_runs(uint64_t (&v)[NV], uint64_t (&ex
 }
 
 // Both kernels walk the entries in tiles of 4096 — four consecutive entries per thread, loads of the next tile issued before
-// the block scan of the current one — so that a 12 k-entry list is three short rounds of coalesced traffic. (The first
-// version gave each thread one contiguous run of n / 1024 entries: twelve dependent, uncoalesced loads deep, 30 us and
-// 22 us of a 115 us read; profiles/r02_launches_step_kernels.md.)
+// the block scan of the current one — so that a 12 k-entry list is three short rounds of coalesced traffic. (One
+// contiguous run of n / 1024 entries per thread would be twelve dependent, uncoalesced loads deep.)
 constexpr uint32_t kPlanPer = 4, kPlanTile = 1024 * kPlanPer;
 
 // counts2[2i] = rows of entry i that survived (MODE_REFINE's count). Writes, for every entry: row_base (rows before it),

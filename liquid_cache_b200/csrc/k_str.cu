@@ -1,4 +1,4 @@
-// k_str.cu — byte-view (dictionary + FSST) columns on sm_100a: predicates and get-with-selection.
+// k_str.cu — byte-view (dictionary + FSST) columns on sm_90a: predicates and get-with-selection.
 //
 // Reference semantics restated (all under /root/reference/src/core/src/liquid_array/byte_view_array/):
 //   try_eval_predicate            mod.rs:357-362, helpers.rs:44-92
@@ -8,7 +8,7 @@
 //   dictionary -> rows            comparisons.rs:325-347
 //   filter / to_arrow_array       mod.rs:266-290, 421-424; helpers.rs:14-64; ../raw/fsst_buffer.rs:88-119, 642-663
 //
-// Design (B200): one CTA per entry. Two TMA bulk copies are issued up front: (A) header + dictionary
+// Design (H100): one CTA per entry. Two TMA bulk copies are issued up front: (A) header + dictionary
 // metadata (shared prefix, 8-byte prefix keys, fingerprints, offset residuals), (B) validity + u16
 // keys. Phase 1 evaluates the predicate ONCE PER DICTIONARY ENTRY on the encoded form (prefix keys /
 // fingerprints first, FSST codes walked only for the candidates that survive) into a bitmap in shared
@@ -378,7 +378,7 @@ __device__ __forceinline__ bool like_trip(const View& v, const uint16_t* s_cand,
   } else {
     // fast path (no escape in any lane's word): plain table steps. (Tried and dropped: an 8-word bitmap of the codes
     // that cannot touch the match state, to skip their 16-byte rows — fewer bank conflicts, but the extra lookup
-    // cost more than it saved: 0.887 vs 0.828 ms on the same GPU.)
+    // cost more than it saved.)
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       if (static_cast<uint32_t>(k) < cnt) {
@@ -478,7 +478,7 @@ __device__ __forceinline__ void str_scan_body(const StrView& v, const EntryIo& w
   // measurement aid (pred.prof): thread 0 stamps the phase boundaries with the SM clock
   long long t_prev = t_start;
   auto stamp = [&](int slot) {
-#ifdef LC_PHASE_PROF  // build with -DLC_PHASE_PROF for the per-phase cycle split (profiles/r01_k_str_scan_phases.txt)
+#ifdef LC_PHASE_PROF  // build with -DLC_PHASE_PROF for the per-phase cycle split (reported by bench.py)
     if (pred.prof && threadIdx.x == 0) {
       const long long t = clock64();
       atomicAdd(&pred.prof[4 + slot], static_cast<unsigned long long>(t - t_prev));
@@ -853,8 +853,7 @@ k_str_scan(ScanIo io, StrPredDesc pred, uint32_t stage_cap, uint32_t dict_words,
 //
 // One WARP per entry, no block-wide phase: an entry is a chain of short dependent steps (header -> gate loads -> a
 // handful of code walks -> 1 KB of output), and a CTA that takes them together waits at every barrier for its slowest
-// lane (ncu r02, the CTA-per-entry form: `No Eligible` 66 %, a third of all samples at the barrier behind the walk,
-// DRAM 31 %). Independent warps keep 8 x as many entries in flight per SM and a walking lane stalls only its own warp.
+// lane. Independent warps keep 8 x as many entries in flight per SM and a walking lane stalls only its own warp.
 // The CTA's warps take neighbouring entries (one column chunk = one FSST symbol table, read through L1), each
 // warp prefetches the next entry's header word and the blob pointer of the one after (registers), fingerprints and
 // trigram sets stream from global memory with coalesced / sector-sized loads, four stripes of 32 values in flight.
@@ -1411,7 +1410,7 @@ __device__ __forceinline__ void str_lengths_entry(const StrGatherIo& g, uint32_t
 // Host-planned gets launch one CTA per entry (per_cta = 1, no k_hint). Device-planned reads do not know on the host which
 // entries have rows, so a CTA takes a RANGE of entries, looks at their survivor counts in one coalesced round and leaves
 // at once when none of them is its business — the common case of a selective scan, where every batch with survivors has a
-// handful and belongs to k_str_lengths_sparse (12 207 one-entry CTAs that only exit cost 15 us of a 115 us read).
+// handful and belongs to k_str_lengths_sparse (12 207 one-entry CTAs that only exit are not free).
 __global__ void __launch_bounds__(256) k_str_lengths(StrGatherIo g, uint32_t stage_cap, uint32_t n_entries, uint32_t per_cta) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   ScanSmem* sm = reinterpret_cast<ScanSmem*>(smem_raw);
@@ -1440,8 +1439,7 @@ __global__ void __launch_bounds__(256) k_str_lengths(StrGatherIo g, uint32_t sta
 }
 
 // A selective scan leaves one or two rows in most of the batches it leaves any in (the bench column: 3 971 rows in 3 400 of
-// 12 207 batches). Staging 30 KB of entry head and synchronising a CTA for that is all overhead (k_str_lengths: 81 us for
-// those 3 400 entries), so such entries get ONE WARP each, reading only what the rows need: the selection words, the key,
+// 12 207 batches). Staging 30 KB of entry head and synchronising a CTA for that is all overhead, so such entries get ONE WARP each, reading only what the rows need: the selection words, the key,
 // its PrefixKey (length byte) and its two offsets. Lists without nulls only (the device-planned read's precondition).
 __global__ void __launch_bounds__(256) k_str_lengths_sparse(StrGatherIo g, uint32_t n_entries) {
   const uint32_t lane = threadIdx.x & 31u;
@@ -1717,7 +1715,7 @@ __global__ void __launch_bounds__(256) k_str_decode_sparse(StrGatherIo g, uint32
 //
 // The device-planned read above is six dependent launches (row plan, lengths x 2, byte plan, decode x 2): right for reads
 // that move data, but a selective LIKE leaves a handful of rows per batch and the read then costs more than the predicate
-// (measured: 0.102 ms of launches and drains behind a 0.093 ms k_str_like). Where each entry's rows and bytes start is a
+// (launches and drains). Where each entry's rows and bytes start is a
 // prefix sum over the entries; here it is a single-pass chained scan (decoupled look-back) across the CTAs of the same
 // kernel that decodes: a CTA takes eight entries (a warp each), sizes their survivors, publishes its (rows, bytes)
 // aggregate, reads its predecessors' until it meets an inclusive prefix, and writes. CTAs take their position from a ticket
@@ -1823,7 +1821,7 @@ __device__ __forceinline__ unsigned long long warp_excl_scan64(unsigned long lon
 // A CTA takes 32 consecutive entries, four per warp: a selective scan leaves most of them without a survivor, and a warp
 // that steps over its empty entries keeps the grid within ONE wave of the GPU for a 12 k-entry list (382 CTAs). That matters
 // because nothing can be written before every predecessor has sized its survivors — with one entry per warp the kernel ran
-// as three waves of 25 us, each waiting for its slowest chain of dependent loads (ncu: 2.1 M polls of predecessors' words).
+// as three waves, each waiting for its slowest chain of dependent loads (polls of predecessors' status words).
 constexpr uint32_t kOpPerWarp = 4, kOpPerCta = 8u * kOpPerWarp;
 
 __global__ void __launch_bounds__(256) k_str_read_onepass(StrGatherIo g, uint32_t n_entries, unsigned long long cap_rows,

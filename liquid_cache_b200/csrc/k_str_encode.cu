@@ -403,7 +403,7 @@ cudaError_t launch_str_encode(const StrEncIo& io, cudaStream_t s) {
   const uint32_t n = io.n;
   if (n) {
     const uint32_t grid = (n + 255u) / 256u;
-    k_dict_insert<<<grid < 1184u ? grid : 1184u, 256, 0, s>>>(io);
+    k_dict_insert<<<grid < kGridStrideCap ? grid : kGridStrideCap, 256, 0, s>>>(io);
   }
   k_dict_finish<<<1, 1024, 0, s>>>(io);
   const uint32_t ugrid = n ? (n + 127u) / 128u : 1u;  // U <= n is only known on the device

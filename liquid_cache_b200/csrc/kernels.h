@@ -1,4 +1,4 @@
-// kernels.h — work-item structs and launchers of the sm_100a kernels (host-visible side).
+// kernels.h — work-item structs and launchers of the sm_90a kernels (host-visible side).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -10,6 +10,8 @@ namespace lc {
 // Shared-memory budget of the scan kernels: a fixed control area + the staged entry blob.
 constexpr uint32_t kScanFixedSmem = 4608;
 constexpr uint32_t kStageCap = 100 * 1024;  // entries larger than this are read straight from global
+// Grid of the grid-stride element-wise kernels: 8 resident 256-thread CTAs on each of an H100 SXM's 132 SMs.
+constexpr uint32_t kGridStrideCap = 132u * 8u;
 
 enum ScanMode : int32_t {
   MODE_DECODE = 0,  // to_arrow_array / filter: values (+validity) of the selected rows

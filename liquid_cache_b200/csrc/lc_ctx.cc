@@ -338,7 +338,7 @@ std::shared_ptr<lc_ctx::CodecSlot> lc_ctx::codec_slot(uint64_t scope) {
 extern "C" {
 
 const char* lc_last_error(void) { return get_error(); }
-const char* lc_version(void) { return "liquid_cache_b200 0.1 (sm_100a)"; }
+const char* lc_version(void) { return "liquid_cache_b200 0.1 (sm_90a)"; }
 
 int lc_ctx_create(int device_id, uint64_t hbm_budget_bytes, lc_ctx** out) {
   if (!out) {
@@ -361,8 +361,8 @@ int lc_ctx_create(int device_id, uint64_t hbm_budget_bytes, lc_ctx** out) {
   LC_CUDA_OK(cudaSetDevice(device_id));
   cudaDeviceProp prop;
   LC_CUDA_OK(cudaGetDeviceProperties(&prop, device_id));
-  if (prop.major != 10) {
-    set_error("device %d is sm_%d%d; this library ships sm_100a code only", device_id, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device %d is sm_%d%d; this library ships sm_90a code only", device_id, prop.major, prop.minor);
     return LC_ERR_NO_DEVICE;
   }
   lc_ctx* ctx = new lc_ctx();

@@ -1,6 +1,6 @@
 """SASS mnemonic census of every kernel in liquid_cache_b200/lib/liblc_gpu.so (cuobjdump -sass): which kernels stage by TMA
 (UBLKCP + SYNCS), which stream with vector loads (LDG.E.128 / .64), where shared memory, votes, shuffles, atomics and spills
-(STL / LDL) sit. Run here after a build:  python profiles/sass_census.py > profiles/r02_sass_census.txt"""
+(STL / LDL) sit. Run here after a build:  python profiles/sass_census.py > sass_census.txt"""
 import collections
 import os
 import re
@@ -45,7 +45,7 @@ def main():
         elif op.startswith("BAR"): c["BAR"] += 1
         elif op.startswith("LDL"): c["LDL"] += 1
         elif op.startswith("STL"): c["STL"] += 1
-    print(f"# {os.path.relpath(LIB, ROOT)}: static SASS instruction counts per kernel (sm_100a)")
+    print(f"# {os.path.relpath(LIB, ROOT)}: static SASS instruction counts per kernel (sm_90a)")
     print("kernel".ljust(58) + " ".join(c.rjust(9) for c in COLS))
     for fn, c in counts.items():
         name = demangle(fn)

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine with one)")
     if os.environ.get("LC_FAKE_NATIVE") == "1":
         # dry run of the GPU tests' Python half on a machine without a GPU: the CPU oracle stands in for liblc_gpu.so
         # (tests/fake_native.py; proves nothing about the device code)

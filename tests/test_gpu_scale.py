@@ -10,8 +10,8 @@ handful of matching rows. Checked on the whole column:
   * get-with-selection of the survivors = the Arrow filter of the same rows, bit for bit
   * encode -> decode round trip of sampled entries (insert, then get of every row) and a checksum of checksums over
     the whole integer column (sum of the decoded values of all survivors, wrapping, = numpy's)
-LC_SCALE_ROWS shrinks the workload for quick runs (default: the 100 M rows bench.py uses; ~20 s per test on a B200 box,
-nearly all of it generating the synthetic input).
+LC_SCALE_ROWS shrinks the workload for quick runs (default: the 100 M rows bench.py uses; nearly all of a
+test's time goes to generating the synthetic input).
 """
 import os
 

@@ -2,7 +2,7 @@
 eval_predicate builders, LiquidExpr) driven by a C++ program that replays the reference's quick-start examples
 (/root/reference/README.md:43-88, src/core/README.md:17-104) — tests/cpp/quickstart.cc, compiled with g++ against
 include/lc_gpu.h and the in-tree liblc_gpu.so. Without a CUDA device the program must stop at the first call with the
-library's "no CPU fallback" error (exit code 3); on a B200 every published answer must come out (exit code 0)."""
+library's "no CPU fallback" error (exit code 3); on an H100 every published answer must come out (exit code 0)."""
 import os
 import subprocess
 
