@@ -139,7 +139,7 @@ def run_sweep(cache, rows: int, steps: int, warmup: int, rank: int = 0, world: i
     import numpy as np
     import pyarrow as pa
 
-    from liquid_cache_b200 import CacheExpression, LiquidExpr, parquet_array_id
+    from liquid_cache_b200 import CacheExpression, Column, InListExpr, LiquidExpr, Literal, parquet_array_id
     from liquid_cache_b200 import _native as N
     from synth.hits import HitsSample
 
@@ -225,14 +225,21 @@ def run_sweep(cache, rows: int, steps: int, warmup: int, rank: int = 0, world: i
         words[nz] = np.packbits(bits.reshape(len(nz), 32), axis=1, bitorder="little").view(np.uint32).reshape(-1)
         scan.load_selections(words)
 
+    # q40's IN conjunct is also run as a device filter (LC_OP_IN) when the scan evaluates InListExpr: the native scan does
+    # (`filter_native` is the sign of it); the comparison / LIKE-only CPU test double does not
+    device_in = hasattr(scan, "filter_native")
     trace_q = os.environ.get("LC_SWEEP_TRACE")  # diagnosis: wall clock per conjunct of one query (synchronises after each)
 
-    def run_query(conj, proj, to_host, want_counts=False, q=None):
+    def run_query(conj, proj, to_host, want_counts=False, q=None, in_on_device=False):
         scan.reset()
         for column, op, lit in conj:
             lit = conjunct_literal(lit)
             t_c = time.perf_counter()
-            if op == "in":
+            if op == "in" and in_on_device:
+                # the same conjunct as a device InListExpr (LC_OP_IN): the reference's LiquidExpr would refuse it
+                expr = LiquidExpr.new_unchecked(InListExpr(Column(column, 0), tuple(Literal(v) for v in lit)))
+                scan.filter(handles[column], expr, types[column])
+            elif op == "in":
                 host_fallback(column, op, lit)
             else:
                 expr = LiquidExpr.try_new(make_expr(column, op, lit, types[column]), types[column], CacheExpression.SubstringSearch)
@@ -310,16 +317,38 @@ def run_sweep(cache, rows: int, steps: int, warmup: int, rank: int = 0, world: i
                                   "running selection, over the query's device time (all launches, host gaps included)"}}
         if q in NOTES:
             r["note"] = NOTES[q]
+        if device_in and any(op == "in" for _c, op, _l in conj):
+            # the IN conjunct on the device as well (the host path above stays, so the sweep totals compare with earlier runs)
+            d_counts, d_total, _ = run_query(conj, proj, False, want_counts=True, in_on_device=True)
+            d_ok = bool(np.array_equal(np.asarray(d_counts[:n_check], dtype=np.int64), expected[repr(conj)][:n_check]))
+            d_ms = []
+            for _ in range(steps):
+                start, stop = timer()
+                start()
+                run_query(conj, proj, False, in_on_device=True)
+                d_ms.append(stop())
+            d_e2e = []
+            for _ in range(max(1, steps // 2)):
+                t0 = time.perf_counter()
+                run_query(conj, proj, True, in_on_device=True)
+                d_e2e.append((time.perf_counter() - t0) * 1e3)
+            r["device_in_list"] = {"ms": float(np.median(d_ms)), "e2e_ms": float(np.median(d_e2e)), "rows_out": int(d_total),
+                                   "counts_match_arrow": d_ok}
         results.append(r)
         if log:
             log(f"q{q}: {r['ms']:.3f} ms device, {r['e2e_ms']:.3f} ms e2e, {total} rows, parity {ok}")
     scan.close()
     total_ms = sum(r["ms"] for r in results)
     total_e2e = sum(r["e2e_ms"] for r in results)
+    # the same totals with the device IN-list variant in place of the host path
+    total_ms_dev = sum(r["device_in_list"]["ms"] if "device_in_list" in r else r["ms"] for r in results)
+    total_e2e_dev = sum(r["device_in_list"]["e2e_ms"] if "device_in_list" in r else r["e2e_ms"] for r in results)
     touched = [r for r in results if r.get("conjuncts", 0) + r.get("projected", 0) > 0]
     return {"rows_local": rows_local, "n_entries": n_entries, "setup_seconds": setup_s, "insert_seconds": insert_s, "queries": results,
-            "sweep_ms": total_ms, "sweep_e2e_ms": total_e2e, "queries_touching_columns": len(touched),
-            "all_counts_match_arrow": all(r.get("counts_match_arrow", True) for r in results),
+            "sweep_ms": total_ms, "sweep_e2e_ms": total_e2e, "sweep_ms_device_in_list": total_ms_dev,
+            "sweep_e2e_ms_device_in_list": total_e2e_dev, "queries_touching_columns": len(touched),
+            "all_counts_match_arrow": all(r.get("counts_match_arrow", True) and r.get("device_in_list", {}).get("counts_match_arrow", True)
+                                          for r in results),
             "literals_from_sample": {k: int(v) for k, v in lits.items()}}
 
 
@@ -384,6 +413,8 @@ def main(args, rank, world, local_rank):
                        "literals_from_sample": res["literals_from_sample"], "slowest_queries": [{"q": r["q"], "ms": r["ms"]} for r in slow],
                        "parallelism": f"entries sharded by EntryID over {world} GPU(s), no data-path collective"},
             "e2e": {"value": scanned / (sweep_e2e / 1e3) / 1e6, "unit": "Mrows/s", "ms_per_step": sweep_e2e},
+            # rank 0's totals with q40's IN conjunct evaluated on the device instead of by the host path
+            "device_in_list": {"ms_per_step": res["sweep_ms_device_in_list"], "e2e_ms_per_step": res["sweep_e2e_ms_device_in_list"]},
             "queries": res["queries"], "peak_source": peak_src, "hbm_peak_gbs": peak, "clocks": clk,
         }
         print(json.dumps(line))

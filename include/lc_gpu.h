@@ -96,8 +96,23 @@ typedef enum lc_op {
   LC_OP_LIKE = 6,        /* LikeExpr / LikeMatch; literal is the SQL pattern WITH its % signs */
   LC_OP_NOT_LIKE = 7,    /* negated LikeExpr / NotLikeMatch                                    */
   LC_OP_CONST_TRUE = 8,  /* Literal(Boolean(true))  on a byte-like column (helpers.rs:72-78)   */
-  LC_OP_CONST_FALSE = 9
+  LC_OP_CONST_FALSE = 9,
+  /* `col [NOT] IN (v1, ..., vn)`: DataFusion's InListExpr over a list without nulls. The reference's LiquidExpr does
+   * not admit it (the caller decodes and lets DataFusion evaluate); this library evaluates it on the device.
+   *   lit_len   number of list values (0 = empty list: false for IN, true for NOT IN on every valid row)
+   *   lit_kind  LC_LIT_I64 / LC_LIT_U64: lit_bytes holds lit_len little-endian 8-byte integers (no alignment needed);
+   *             LC_LIT_BYTES: Arrow's Utf8 layout in one buffer, int32 offsets[lit_len + 1] (offsets[0] == 0,
+   *             non-decreasing) followed by offsets[lit_len] value bytes (LC_ERR_INVALID when malformed)
+   * Null rows give null (value bit 0, validity bit 0); lc_scan_filter turns them into false, as for every conjunct.
+   * Duplicates do not matter. Accepted on integer / date / timestamp and byte-view entries; float, decimal, squeezed
+   * entries and lists over the caps below return LC_ERR_UNSUPPORTED_EXPR and write nothing. */
+  LC_OP_IN = 10,
+  LC_OP_NOT_IN = 11
 } lc_op;
+
+/* Largest IN list evaluated on the device: values per list, and value bytes of an LC_LIT_BYTES list. */
+#define LC_IN_LIST_MAX_VALUES 256
+#define LC_IN_LIST_MAX_BYTES 16384
 
 /* CacheExpression hint (cache/expressions.rs:38-53) — only SUBSTRING_SEARCH changes the encoding
  * (it turns on the per-unique 32-bit fingerprints, transcode.rs:165). */

@@ -7,11 +7,11 @@ without the built library, or calling into it without an H100, raises: there is 
 from . import _native
 from .cache import (EntryID, EvaluatePredicate, Get, GpuLiquidArray, Insert, LiquidCache, LiquidCacheBuilder, Scan,
                     parquet_array_id, selection_bits)
-from .expr import (BinaryExpr, CacheExpression, CastColumnExpr, CastExpr, Column, DynamicFilterPhysicalExpr, LikeExpr,
-                   LiquidExpr, Literal, ScalarFunctionExpr, TryCastExpr)
+from .expr import (BinaryExpr, CacheExpression, CastColumnExpr, CastExpr, Column, DynamicFilterPhysicalExpr, InListExpr,
+                   LikeExpr, LiquidExpr, Literal, ScalarFunctionExpr, TryCastExpr)
 
 __all__ = [
     "EntryID", "EvaluatePredicate", "Get", "GpuLiquidArray", "Insert", "LiquidCache", "LiquidCacheBuilder", "Scan",
     "parquet_array_id", "selection_bits", "BinaryExpr", "CacheExpression", "CastColumnExpr", "CastExpr", "Column",
-    "DynamicFilterPhysicalExpr", "LikeExpr", "LiquidExpr", "Literal", "ScalarFunctionExpr", "TryCastExpr",
+    "DynamicFilterPhysicalExpr", "InListExpr", "LikeExpr", "LiquidExpr", "Literal", "ScalarFunctionExpr", "TryCastExpr",
 ]

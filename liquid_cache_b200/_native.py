@@ -22,6 +22,8 @@ LC_ERR_OOM = -7
 LC_ERR_NO_DEVICE = -8
 
 OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT, OP_GE, OP_LIKE, OP_NOT_LIKE, OP_CONST_TRUE, OP_CONST_FALSE = range(10)
+OP_IN, OP_NOT_IN = 10, 11  # InListExpr (lit_len values in lit_bytes)
+IN_LIST_MAX_VALUES, IN_LIST_MAX_BYTES = 256, 16384  # LC_IN_LIST_MAX_VALUES / LC_IN_LIST_MAX_BYTES
 HINT_NONE, HINT_PREDICATE, HINT_SUBSTRING_SEARCH = 0, 1, 2
 HINT_EXTRACT = {"Year": 3, "Month": 4, "Day": 5, "DayOfWeek": 6}  # CacheExpression::ExtractDate32 { field }
 LIT_I64, LIT_U64, LIT_BYTES, LIT_I128, LIT_F64 = 0, 1, 2, 3, 4

@@ -373,8 +373,8 @@ __device__ __forceinline__ void int_bits_fast_w_dispatch(uint32_t W, const Entry
   }
 }
 
-template <typename U, int MODE>
-__device__ __forceinline__ bool int_scan_entry(const EntryIo& w, const IntPredDesc& pred, const uint8_t* base,
+template <typename U, int MODE, bool SET>
+__device__ __forceinline__ bool int_scan_entry(const EntryIo& w, const IntPredDesc& pred, const IntInList& in, const uint8_t* base,
                                                bool staged, ScanSmem* sm, uint32_t& tab_key, uint32_t* fast_cnt) {
   constexpr uint32_t T = FL<U>::T;
   const IntHeader* h = reinterpret_cast<const IntHeader*>(base);
@@ -382,7 +382,7 @@ __device__ __forceinline__ bool int_scan_entry(const EntryIo& w, const IntPredDe
   const U ref = static_cast<U>(h->reference);
   int32_t kind = UC_TRUE;
   uint64_t thr64 = 0;
-  if (MODE != MODE_DECODE) plan_int_pred(h, pred, &kind, &thr64);
+  if (MODE != MODE_DECODE && !SET) plan_int_pred(h, pred, &kind, &thr64);
   const uint8_t* packed = base + h->packed_off;
   const uint32_t* valid = h->has_nulls ? reinterpret_cast<const uint32_t*>(base + h->validity_off) : nullptr;
   const uint32_t chunk_bytes = 128u * W;
@@ -396,6 +396,31 @@ __device__ __forceinline__ bool int_scan_entry(const EntryIo& w, const IntPredDe
     auto emit = [&](uint32_t, uint32_t dst, uint32_t, uint32_t) { out_vals[dst] = ref; };
     tab_key = 0;
     scan_entry_rows<MODE>(w.sel, n, valid, nulls, out_bits, w.out_valid, w.counts, sm, cmp, emit);
+    return false;
+  }
+  if constexpr (SET) {
+    // IN lists on the general row loop, every shape (k_int_bits is their fast path): plan_int_in per entry; a set test
+    // looks the packed value up among the slice's offsets in global memory
+    tab_key = 0;
+    URange<uint64_t> g;
+    uint32_t a = 0, b = 0;
+    const bool set = plan_int_in<uint64_t>(h, pred.op, in, &g, &a, &b);
+    const uint64_t ref64 = window_ref(h);
+    const uint32_t mask = W >= 32u ? 0xffffffffu : ((1u << W) - 1u);
+    auto val = [&](uint32_t c, uint32_t j) -> uint64_t {
+      const uint8_t* chunk = packed + static_cast<size_t>(c) * chunk_bytes;
+      if (T == 64 && W > 32u) return fl_step64_hi(reinterpret_cast<const uint32_t*>(chunk), j, lane, W);
+      if (T == 64) return fl_step64_lo(reinterpret_cast<const uint32_t*>(chunk), j, lane, W, mask);
+      if (T == 32) return fl_step32(reinterpret_cast<const uint32_t*>(chunk), j, lane, W, mask);
+      return fl_step_small<U>(reinterpret_cast<const U*>(chunk), j, lane, W, mask);
+    };
+    auto cmp = [&](uint32_t, uint32_t c, uint32_t j) -> bool {
+      const uint64_t u = val(c, j);
+      const bool hit = set ? in_sorted<uint64_t>(u, b - a, [&](uint32_t i) { return in.v[a + i] - ref64; }) : (u - g.lo) <= g.span;
+      return hit != g.neg;
+    };
+    auto emit = [&](uint32_t, uint32_t, uint32_t, uint32_t) {};
+    scan_entry_rows<MODE>(w.sel, n, valid, nulls, out_bits, w.out_valid, w.counts, sm, cmp, emit, FLOrder<U>());
     return false;
   }
   // full-length bit outputs from a staged entry: no compaction needed
@@ -446,8 +471,8 @@ __device__ __forceinline__ bool int_scan_entry(const EntryIo& w, const IntPredDe
 // warps work on the entry staged in one shared-memory buffer, thread 0 has already issued the bulk copy of the
 // CTA's next entry into the other buffer (its own mbarrier, phase = use count parity). Entry fetch latency is
 // hidden behind compute instead of being paid once per 8192 rows.
-template <int MODE>
-__global__ void __launch_bounds__(256, 4) k_int_scan(ScanIo io, IntPredDesc pred, uint32_t n_entries, uint32_t stage_bytes) {
+template <int MODE, bool SET>
+__global__ void __launch_bounds__(256, 4) k_int_scan(ScanIo io, IntPredDesc pred, uint32_t n_entries, uint32_t stage_bytes, IntInList in) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   ScanSmem* sm = reinterpret_cast<ScanSmem*>(smem_raw);
   uint8_t* stage0 = smem_raw + kScanFixedSmem;
@@ -511,10 +536,10 @@ __global__ void __launch_bounds__(256, 4) k_int_scan(ScanIo io, IntPredDesc pred
     const IntHeader* h = reinterpret_cast<const IntHeader*>(base);
     const EntryIo w = resolve_io_slot(io, sm->io_slot[buf], e, MODE == MODE_DECODE ? h->tbits / 8u : 4u);
     switch (h->tbits) {
-      case 8: pending = int_scan_entry<uint8_t, MODE>(w, pred, base, staged, sm, tab_key, &sm->fcnt[buf]); break;
-      case 16: pending = int_scan_entry<uint16_t, MODE>(w, pred, base, staged, sm, tab_key, &sm->fcnt[buf]); break;
-      case 32: pending = int_scan_entry<uint32_t, MODE>(w, pred, base, staged, sm, tab_key, &sm->fcnt[buf]); break;
-      default: pending = int_scan_entry<uint64_t, MODE>(w, pred, base, staged, sm, tab_key, &sm->fcnt[buf]); break;
+      case 8: pending = int_scan_entry<uint8_t, MODE, SET>(w, pred, in, base, staged, sm, tab_key, &sm->fcnt[buf]); break;
+      case 16: pending = int_scan_entry<uint16_t, MODE, SET>(w, pred, in, base, staged, sm, tab_key, &sm->fcnt[buf]); break;
+      case 32: pending = int_scan_entry<uint32_t, MODE, SET>(w, pred, in, base, staged, sm, tab_key, &sm->fcnt[buf]); break;
+      default: pending = int_scan_entry<uint64_t, MODE, SET>(w, pred, in, base, staged, sm, tab_key, &sm->fcnt[buf]); break;
     }
     if (threadIdx.x < 3u) sm->io_slot[buf ^ 1u][threadIdx.x] = nx_io;
     else if (threadIdx.x < 5u) sm->ref_slot[threadIdx.x - 3u] = nx_io;
@@ -524,7 +549,7 @@ __global__ void __launch_bounds__(256, 4) k_int_scan(ScanIo io, IntPredDesc pred
 }
 
 cudaError_t launch_int_scan(int mode, uint32_t n_entries, const ScanIo& io, const IntPredDesc& pred,
-                            uint32_t max_blob_bytes, cudaStream_t s) {
+                            uint32_t max_blob_bytes, cudaStream_t s, const IntInList& in) {
   if (n_entries == 0) return cudaSuccess;
   const uint32_t stage = max_blob_bytes <= kStageCap ? ((max_blob_bytes + 127u) & ~127u) : 0u;
   // Two stage buffers (prefetch of the CTA's next entry) only while >= 3 CTAs still fit on an SM; wide columns
@@ -535,15 +560,11 @@ cudaError_t launch_int_scan(int mode, uint32_t n_entries, const ScanIo& io, cons
   static int n_sm = 132;
   if (!attr_set) {
     cudaError_t e;
-    e = cudaFuncSetAttribute(k_int_scan<MODE_DECODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kScanFixedSmem + 2 * kStageCap);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_int_scan<MODE_PRED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kScanFixedSmem + 2 * kStageCap);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_int_scan<MODE_REFINE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             kScanFixedSmem + 2 * kStageCap);
-    if (e != cudaSuccess) return e;
+    for (auto k : {k_int_scan<MODE_DECODE, false>, k_int_scan<MODE_PRED, false>, k_int_scan<MODE_REFINE, false>,
+                   k_int_scan<MODE_PRED, true>, k_int_scan<MODE_REFINE, true>}) {
+      e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanFixedSmem + 2 * kStageCap);
+      if (e != cudaSuccess) return e;
+    }
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
@@ -557,10 +578,17 @@ cudaError_t launch_int_scan(int mode, uint32_t n_entries, const ScanIo& io, cons
     grid = static_cast<uint32_t>(n_sm) * per_sm;
     if (grid > n_entries) grid = n_entries;
   }
+  const bool set = mode != MODE_DECODE && (pred.op == kOpIn || pred.op == kOpNotIn);
   switch (mode) {
-    case MODE_DECODE: k_int_scan<MODE_DECODE><<<grid, 256, smem, s>>>(io, pred, n_entries, stage); break;
-    case MODE_PRED: k_int_scan<MODE_PRED><<<grid, 256, smem, s>>>(io, pred, n_entries, stage); break;
-    default: k_int_scan<MODE_REFINE><<<grid, 256, smem, s>>>(io, pred, n_entries, stage); break;
+    case MODE_DECODE: k_int_scan<MODE_DECODE, false><<<grid, 256, smem, s>>>(io, pred, n_entries, stage, in); break;
+    case MODE_PRED:
+      if (set) k_int_scan<MODE_PRED, true><<<grid, 256, smem, s>>>(io, pred, n_entries, stage, in);
+      else k_int_scan<MODE_PRED, false><<<grid, 256, smem, s>>>(io, pred, n_entries, stage, in);
+      break;
+    default:
+      if (set) k_int_scan<MODE_REFINE, true><<<grid, 256, smem, s>>>(io, pred, n_entries, stage, in);
+      else k_int_scan<MODE_REFINE, false><<<grid, 256, smem, s>>>(io, pred, n_entries, stage, in);
+      break;
   }
   return cudaGetLastError();
 }

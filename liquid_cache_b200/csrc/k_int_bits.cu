@@ -45,14 +45,37 @@ __host__ __device__ constexpr uint32_t chunks_in_flight() {
   return regs <= 10u ? 4u : (regs <= 20u ? 2u : 1u);
 }
 
+// Membership of one packed value in a warp's set. Not inlined: the 32 unrolled steps of every (T, W) instantiation call it
+// instead of each carrying a copy of the search (which multiplies the build time of this file for no gain in speed).
+__device__ __noinline__ bool in_warp_set(uint32_t u, const uint32_t* set, uint32_t n) {
+  return in_sorted<uint32_t>(u, n, [&](uint32_t i) { return set[i]; });
+}
+
+// The per-row test of a chunk, before negation: the range of a comparison, or (IN lists, SET) membership in the entry's
+// in-window list values, ascending packed offsets in the warp's slice of shared memory (set_n == 0: the entry's plan
+// lowered to a range after all).
+template <bool SET>
+struct RowTest {
+  URange<uint32_t> g;
+  const uint32_t* set;
+  uint32_t set_n;
+  __device__ __forceinline__ bool operator()(uint32_t u) const {
+    if constexpr (SET) {
+      if (set_n) return in_warp_set(u, set, set_n);
+    }
+    return (u - g.lo) <= g.span;
+  }
+};
+
 // One group of chunks [c0, c1) of an entry: every chunk's mask word is finished (negation, validity,
 // selection, tail), stored, and its survivors counted. Returns the survivors of the group (per lane, to be summed).
 // A group that ends inside a CH-wide step (entries whose chunk count is not a multiple of CH) re-reads its last chunk
 // in the surplus slots and drops their words.
-template <uint32_t T, uint32_t W>
+template <uint32_t T, uint32_t W, bool SET>
 __device__ __forceinline__ uint32_t bits_group(const uint8_t* packed, uint32_t c0, uint32_t c1, uint32_t lane, uint32_t ordl,
-                                               const URange<uint32_t>& g, uint32_t n, const uint32_t* sel, const uint32_t* valid,
+                                               const RowTest<SET>& rt, uint32_t n, const uint32_t* sel, const uint32_t* valid,
                                                uint32_t* out_bits, uint32_t* out_valid, uint32_t* strip) {
+  const URange<uint32_t>& g = rt.g;
   constexpr uint32_t CH = chunks_in_flight<T, W>();
   using G = BregGeom<T, W>;
   const uint32_t n_words = (n + 31u) >> 5;
@@ -86,7 +109,7 @@ __device__ __forceinline__ uint32_t bits_group(const uint8_t* packed, uint32_t c
 #pragma unroll
       for (uint32_t s = 0; s < 32; ++s) {
         const uint32_t u = breg_value<T, W>(a[q], s);
-        const uint32_t cw = __ballot_sync(kFullMask, (u - g.lo) <= g.span);
+        const uint32_t cw = __ballot_sync(kFullMask, rt(u));
         if (lane == 0) strip[s] = cw;
       }
       __syncwarp();
@@ -106,14 +129,14 @@ __device__ __forceinline__ uint32_t bits_group(const uint8_t* packed, uint32_t c
   return survivors;
 }
 
-template <uint32_t T>
+template <uint32_t T, bool SET>
 __device__ __forceinline__ uint32_t bits_group_w(uint32_t W, const uint8_t* packed, uint32_t c0, uint32_t c1, uint32_t lane,
-                                                 uint32_t ordl, const URange<uint32_t>& g, uint32_t n, const uint32_t* sel,
+                                                 uint32_t ordl, const RowTest<SET>& g, uint32_t n, const uint32_t* sel,
                                                  const uint32_t* valid, uint32_t* out_bits, uint32_t* out_valid, uint32_t* strip) {
   switch (W) {
 #define LC_W(k) \
   case k:       \
-    if constexpr (k <= T) return bits_group<T, k>(packed, c0, c1, lane, ordl, g, n, sel, valid, out_bits, out_valid, strip); \
+    if constexpr (k <= T) return bits_group<T, k, SET>(packed, c0, c1, lane, ordl, g, n, sel, valid, out_bits, out_valid, strip); \
     break;
     LC_W(1) LC_W(2) LC_W(3) LC_W(4) LC_W(5) LC_W(6) LC_W(7) LC_W(8) LC_W(9) LC_W(10) LC_W(11) LC_W(12) LC_W(13) LC_W(14) LC_W(15) LC_W(16)
     LC_W(17) LC_W(18) LC_W(19) LC_W(20) LC_W(21) LC_W(22) LC_W(23) LC_W(24) LC_W(25) LC_W(26) LC_W(27) LC_W(28) LC_W(29) LC_W(30) LC_W(31) LC_W(32)
@@ -155,9 +178,14 @@ static_assert(offsetof(IntHeader, n) == 8 && offsetof(IntHeader, reference) == 1
 // chunks), shorter entries have idle tasks. The warps of a CTA take consecutive tasks, i.e. the groups of neighbouring entries. Per task the
 // header is read once and the predicate planned once; the header of the warp's next task and the blob pointer of the
 // one after are already in flight (software pipeline in registers).
-template <int OCC>
-__global__ void __launch_bounds__(256, OCC) k_int_bits(ScanIo io, IntPredDesc pred, uint32_t n_entries, uint32_t gshift, uint32_t cshift, int mode) {
+// SET: IN / NOT IN lists (pred.op, values in `in`), planned per task by plan_int_in's two steps — the warp counts the list
+// values below / inside the entry's window with one vote per 32 values, lower_in_slice picks constant, range or set, and a
+// set is copied into the warp's slice of shared memory as packed offsets. The rows are still read in one pass.
+template <int OCC, bool SET>
+__global__ void __launch_bounds__(256, OCC) k_int_bits(ScanIo io, IntPredDesc pred, uint32_t n_entries, uint32_t gshift, uint32_t cshift, int mode,
+                                                     IntInList in) {
   __shared__ uint32_t s_strip[8][32];  // per warp: the 32 ballots of a chunk, transposed through shared memory
+  __shared__ uint32_t s_set[SET ? 8 : 1][SET ? kInListMaxValues : 1];  // per warp: the set of its current task
   const uint32_t lane = threadIdx.x & 31u;
   uint32_t* strip = s_strip[threadIdx.x >> 5];
   const uint32_t warps_total = gridDim.x * 8u;
@@ -199,10 +227,35 @@ __global__ void __launch_bounds__(256, OCC) k_int_bits(ScanIo io, IntPredDesc pr
       hh.patch_idx_off = h0.sq_lo;
       hh.patch_val_off = h0.sq_hi;
       hh.squeeze_kind = static_cast<uint8_t>(h0.sq_kind & 0xffu);
-      int32_t kind = UC_FALSE;
-      uint64_t thr64 = 0;
-      plan_int_pred(&hh, pred, &kind, &thr64);
-      const URange<uint32_t> g = make_range<uint32_t>(kind, thr64);
+      RowTest<SET> g;
+      g.set = nullptr;
+      g.set_n = 0;
+      if constexpr (SET) {
+        uint32_t below = 0, inside = 0;
+        if (W != 0u) {
+          for (uint32_t i = lane; i < in.n; i += 32u) {
+            const int where = in_value_window(&hh, __ldg(reinterpret_cast<const unsigned long long*>(in.v) + i));
+            below += where < 0 ? 1u : 0u;
+            inside += where == 0 ? 1u : 0u;
+          }
+          below = warp_sum(below);
+          inside = warp_sum(inside);
+        }
+        if (lower_in_slice<uint32_t>(&hh, pred.op, in, below, below + inside, &g.g)) {
+          uint32_t* set = s_set[threadIdx.x >> 5];
+          const uint32_t ref = static_cast<uint32_t>(window_ref(&hh));
+          __syncwarp();  // the previous task's lookups are done
+          for (uint32_t i = lane; i < inside; i += 32u) set[i] = static_cast<uint32_t>(in.v[below + i]) - ref;
+          __syncwarp();
+          g.set = set;
+          g.set_n = inside;
+        }
+      } else {
+        int32_t kind = UC_FALSE;
+        uint64_t thr64 = 0;
+        plan_int_pred(&hh, pred, &kind, &thr64);
+        g.g = make_range<uint32_t>(kind, thr64);
+      }
       uint32_t survivors = 0;
       if (W != 0u) {
         const uint8_t* packed = blob0 + h0.packed_off;
@@ -251,7 +304,7 @@ __global__ void __launch_bounds__(256, OCC) k_int_bits(ScanIo io, IntPredDesc pr
 // The host guarantees: every entry is an integer-shaped blob with tbits in {8,16,32,64}, bit_width <= 32, and the counts
 // array (if any) is zeroed on the stream before this launch.
 cudaError_t launch_int_bits(int mode, uint32_t n_entries, const ScanIo& io, const IntPredDesc& pred, uint32_t max_rows,
-                            cudaStream_t s) {
+                            cudaStream_t s, const IntInList& in) {
   if (n_entries == 0) return cudaSuccess;
   static int n_sm = 0;
   if (!n_sm) {
@@ -267,8 +320,8 @@ cudaError_t launch_int_bits(int mode, uint32_t n_entries, const ScanIo& io, cons
   }();
   static int per_sm = 0;
   if (!per_sm) {
-    cudaError_t e = occ_pref == 4 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_int_bits<4>, 256, 0)
-                                  : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_int_bits<3>, 256, 0);
+    cudaError_t e = occ_pref == 4 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_int_bits<4, false>, 256, 0)
+                                  : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_int_bits<3, false>, 256, 0);
     if (e != cudaSuccess) return e;
     if (per_sm < 1) per_sm = 1;
   }
@@ -287,8 +340,24 @@ cudaError_t launch_int_bits(int mode, uint32_t n_entries, const ScanIo& io, cons
   if (n_tasks > 0x7fffffffull) return cudaErrorInvalidValue;
   const uint32_t need = static_cast<uint32_t>((n_tasks + 7u) / 8u);
   if (grid > need) grid = need;
-  if (occ_pref == 4) k_int_bits<4><<<grid, 256, 0, s>>>(io, pred, n_entries, gshift, cshift, mode);
-  else k_int_bits<3><<<grid, 256, 0, s>>>(io, pred, n_entries, gshift, cshift, mode);
+  const bool set = pred.op == kOpIn || pred.op == kOpNotIn;
+  if (set) {
+    // IN lists: the default 80-register build only (LC_INT_OCC does not apply), which holds 8 KB more shared memory per
+    // CTA: its own residency, the same persistent grid shape
+    static int per_sm_set = 0;
+    if (!per_sm_set) {
+      cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_set, k_int_bits<3, true>, 256, 0);
+      if (e != cudaSuccess) return e;
+      if (per_sm_set < 1) per_sm_set = 1;
+    }
+    uint32_t grid_set = static_cast<uint32_t>(n_sm * per_sm_set);
+    if (grid_set > need) grid_set = need;
+    k_int_bits<3, true><<<grid_set, 256, 0, s>>>(io, pred, n_entries, gshift, cshift, mode, in);
+  } else if (occ_pref == 4) {
+    k_int_bits<4, false><<<grid, 256, 0, s>>>(io, pred, n_entries, gshift, cshift, mode, in);
+  } else {
+    k_int_bits<3, false><<<grid, 256, 0, s>>>(io, pred, n_entries, gshift, cshift, mode, in);
+  }
   return cudaGetLastError();
 }
 

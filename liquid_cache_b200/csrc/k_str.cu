@@ -211,6 +211,21 @@ struct StrPlan {
   uint64_t key_expect;
 };
 
+// The PrefixKey (prefix7 + length, 255 = "255 or more") a dictionary value equal to the needle nd[0..m) has in an entry
+// whose shared prefix is sp[0..spl) (comparisons.rs:33-49). False when the needle does not start with the shared prefix:
+// then no value of the entry can equal it.
+__device__ __forceinline__ bool eq_prefix_key(const uint8_t* nd, uint32_t m, const uint8_t* sp, uint32_t spl, uint64_t* key) {
+  bool has_prefix = m >= spl;
+  for (uint32_t i = 0; has_prefix && i < spl; ++i) has_prefix = nd[i] == sp[i];
+  if (!has_prefix) return false;
+  const uint32_t L = m - spl;
+  uint64_t k = 0;
+  for (uint32_t b = 0; b < (L < 7u ? L : 7u); ++b) k |= static_cast<uint64_t>(nd[spl + b]) << (8u * b);
+  k |= static_cast<uint64_t>(L >= 255u ? 255u : L) << 56;
+  *key = k;
+  return true;
+}
+
 __device__ __forceinline__ void plan_str_pred(const StrView& v, const StrPredDesc& pred, const uint8_t* nd,
                                               StrPlan* out) {
   const int op = pred.op;
@@ -225,17 +240,12 @@ __device__ __forceinline__ void plan_str_pred(const StrView& v, const StrPredDes
     p.flags = (op == LC_OP_CONST_TRUE) ? 1u : 0u;
   } else if (op == LC_OP_EQ || op == LC_OP_NE) {
     const bool neg = (op == LC_OP_NE);
-    bool has_prefix = m >= spl;
-    for (uint32_t i = 0; has_prefix && i < spl; ++i) has_prefix = nd[i] == v.sp[i];
-    if (!has_prefix) {
+    uint64_t k = 0;
+    if (!eq_prefix_key(nd, m, v.sp, spl, &k)) {
       p.flags = neg ? 1u : 0u;  // no value can equal the needle
     } else {
-      const uint32_t L = m - spl;
-      uint64_t k = 0;
-      for (uint32_t b = 0; b < (L < 7u ? L : 7u); ++b) k |= static_cast<uint64_t>(nd[spl + b]) << (8u * b);
-      k |= static_cast<uint64_t>(L >= 255u ? 255u : L) << 56;
       p.key_expect = k;
-      p.kind = (L <= 7u) ? SP_EQ_SHORT : SP_EQ_LONG;
+      p.kind = (m - spl <= 7u) ? SP_EQ_SHORT : SP_EQ_LONG;
       p.flags = neg ? 2u : 0u;
     }
   } else if (op >= LC_OP_LT && op <= LC_OP_GE) {
@@ -260,6 +270,9 @@ __device__ __forceinline__ void plan_str_pred(const StrView& v, const StrPredDes
         p.cmp_len = L7;
       }
     }
+  } else if (op == LC_OP_IN || op == LC_OP_NOT_IN) {  // the needles are planned by all threads (in_list_table)
+    p.kind = SP_IN;
+    p.flags = op == LC_OP_NOT_IN ? 2u : 0u;
   } else {  // LIKE / NOT LIKE
     p.kind = SP_LIKE;
     p.flags = (op == LC_OP_NOT_LIKE ? 2u : 0u) | (v.h->has_fp ? 0u : 4u);
@@ -465,9 +478,74 @@ __device__ __forceinline__ void like_candidates_warp(const View& v, const uint16
   }
 }
 
+// ---- IN lists ---------------------------------------------------------------------------------------
+// Per entry, every needle of the list (pred.needle: int32 offsets[list_n + 1], then the bytes; read from global memory) is
+// planned as `=` plans it: does it start with the shared prefix, and which PrefixKey would an equal value have. Thread t
+// plans needle t; the (key, needle) pairs are then sorted by key in shared memory (bitonic, kInListMaxValues = 256 slots,
+// needles without the prefix and empty slots at the end), so that a dictionary value finds the needles with its own key by
+// one binary search. A key whose length byte is <= 7 belongs to a short needle, and an equal key IS an equal value; a
+// longer key only makes the value a candidate, decided by full_compare against each long needle with that key.
+constexpr uint32_t kInTableBytes = kInListMaxValues * 8u + kInListMaxValues * 2u;
+static_assert(kInListMaxValues == 256u, "one needle per thread of the 256-thread CTA");
+
+__device__ __forceinline__ const int32_t* in_offsets(const StrPredDesc& pred) { return reinterpret_cast<const int32_t*>(pred.needle); }
+__device__ __forceinline__ const uint8_t* in_bytes(const StrPredDesc& pred) { return pred.needle + 4u * (pred.list_n + 1u); }
+
+// returns the number of needles that have the prefix (the sorted prefix of the table)
+__device__ __forceinline__ uint32_t in_list_table(const StrView& v, const StrPredDesc& pred, uint64_t* s_key, uint16_t* s_tag) {
+  const uint32_t t = threadIdx.x;
+  uint64_t key = ~0ull;
+  uint32_t tag = 0xffffu;  // empty slot
+  if (t < pred.list_n) {
+    const int32_t* off = in_offsets(pred);
+    const uint32_t o = static_cast<uint32_t>(off[t]), len = static_cast<uint32_t>(off[t + 1u]) - o;
+    if (eq_prefix_key(in_bytes(pred) + o, len, v.sp, v.h->shared_prefix_len, &key)) {
+      tag = t;
+    } else {
+      key = ~0ull;
+      tag = 0x8000u | t;
+    }
+  }
+  s_key[t] = key;
+  s_tag[t] = static_cast<uint16_t>(tag);
+  const uint32_t n_valid = static_cast<uint32_t>(__syncthreads_count(tag < 0x8000u));
+  for (uint32_t k = 2; k <= kInListMaxValues; k <<= 1) {
+    for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+      const uint32_t l = t ^ j;
+      if (l > t) {
+        const uint64_t ka = s_key[t], kb = s_key[l];
+        const uint16_t ta = s_tag[t], tb = s_tag[l];
+        const bool gt = ka > kb || (ka == kb && ta > tb);
+        if (gt == ((t & k) == 0)) {
+          s_key[t] = kb;
+          s_key[l] = ka;
+          s_tag[t] = tb;
+          s_tag[l] = ta;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  return n_valid;
+}
+
+__device__ __forceinline__ uint32_t in_lower_bound(const uint64_t* s_key, uint32_t n, uint64_t key) {
+  uint32_t lo = 0, len = n;
+  while (len > 0) {
+    const uint32_t half = len >> 1;
+    if (s_key[lo + half] < key) {
+      lo += half + 1u;
+      len -= half + 1u;
+    } else {
+      len = half;
+    }
+  }
+  return lo;
+}
+
 // The body of the predicate kernel, instantiated per address space of the staged sections so that the
-// compiler emits LDS / LDG instead of generic loads.
-template <int MODE>
+// compiler emits LDS / LDG instead of generic loads. IN: the instantiation for IN lists (SP_IN; s_nd holds the table).
+template <int MODE, bool IN>
 __device__ __forceinline__ void str_scan_body(const StrView& v, const EntryIo& w, const StrPredDesc& pred,
                                               ScanSmem* sm, uint64_t* s_sym, uint8_t* s_len, StrPlan* s_plan,
                                               const uint8_t* s_nd, const uint16_t* s_fail, uint32_t* s_dict,
@@ -495,7 +573,11 @@ __device__ __forceinline__ void str_scan_body(const StrView& v, const EntryIo& w
   const int lane = threadIdx.x & 31;
   const int32_t kind = plan.kind;
   const bool neg = (plan.flags & 2u) != 0;
-  const bool needs_table = (kind == SP_EQ_LONG || kind == SP_ORD || kind == SP_LIKE);
+  const bool needs_table = (kind == SP_EQ_LONG || kind == SP_ORD || kind == SP_LIKE || kind == SP_IN);
+  uint64_t* s_in_key = reinterpret_cast<uint64_t*>(const_cast<uint8_t*>(s_nd));
+  uint16_t* s_in_tag = reinterpret_cast<uint16_t*>(s_in_key + kInListMaxValues);
+  uint32_t in_valid = 0;
+  if constexpr (IN) in_valid = in_list_table(v, pred, s_in_key, s_in_tag);  // ends with a barrier
   const bool fast_like = (kind == SP_LIKE) && m <= 31u;
   if (needs_table && v.h->table_ptr != table_cache) {
     // symbol table + step table of this column chunk; a CTA walks consecutive entries, which usually share it
@@ -602,6 +684,15 @@ __device__ __forceinline__ void str_scan_body(const StrView& v, const EntryIo& w
         } else if (kind == SP_EQ_LONG) {
           cand = (key == plan.key_expect);
           res = neg;
+        } else if (IN && kind == SP_IN) {
+          const uint32_t t = in_lower_bound(s_in_key, in_valid, key);
+          const bool hit = t < in_valid && s_in_key[t] == key;
+          if ((key >> 56) <= 7u) {
+            res = hit != neg;  // short needle: the key decides
+          } else {
+            cand = hit;
+            res = neg;
+          }
         } else if (kind == SP_ORD) {
           const uint64_t mask = ~0ull << (8u * (8u - plan.cmp_len));
           const uint64_t a = bswap64(key) & mask;
@@ -646,12 +737,21 @@ __device__ __forceinline__ void str_scan_body(const StrView& v, const EntryIo& w
         bool res;
         if (kind == SP_LIKE) {
           res = contains_needle(v, i, s_sym, s_len, s_nd, s_fail, m);
+        } else if (IN && kind == SP_IN) {
+          const uint64_t key = v.pk[i];
+          const int32_t* off = in_offsets(pred);
+          bool eq = false;
+          for (uint32_t t = in_lower_bound(s_in_key, in_valid, key); !eq && t < in_valid && s_in_key[t] == key; ++t) {
+            const uint32_t j = s_in_tag[t], o = static_cast<uint32_t>(off[j]);
+            eq = full_compare(v, i, s_sym, s_len, in_bytes(pred) + o, static_cast<uint32_t>(off[j + 1u]) - o) == 0;
+          }
+          res = eq != neg;
         } else {
           const int ord = full_compare(v, i, s_sym, s_len, s_nd, m);
           if (kind == SP_EQ_LONG) res = (ord == 0) != neg;
           else res = (op == LC_OP_LT) ? ord < 0 : (op == LC_OP_LE) ? ord <= 0 : (op == LC_OP_GT) ? ord > 0 : ord >= 0;
         }
-        if (kind == SP_EQ_LONG && neg) {
+        if ((kind == SP_EQ_LONG || (IN && kind == SP_IN)) && neg) {
           if (!res) atomicAnd(&s_dict[i >> 5], ~(1u << (i & 31u)));
         } else if (res) {
           atomicOr(&s_dict[i >> 5], 1u << (i & 31u));
@@ -747,7 +847,7 @@ __device__ __forceinline__ void str_scan_body(const StrView& v, const EntryIo& w
 //   result bits | candidate list | staged entry head
 constexpr uint32_t kStrScanTables = 2048u + 256u + 32u + 1024u + 8192u;
 
-template <int MODE>
+template <int MODE, bool IN>
 __global__ void __launch_bounds__(256, 4)
 k_str_scan(ScanIo io, StrPredDesc pred, uint32_t stage_cap, uint32_t dict_words, uint32_t n_entries, uint32_t per_cta) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
@@ -759,7 +859,7 @@ k_str_scan(ScanIo io, StrPredDesc pred, uint32_t stage_cap, uint32_t dict_words,
   SymStep* s_step = reinterpret_cast<SymStep*>(s_M + 256);
   uint8_t* s_nd = reinterpret_cast<uint8_t*>(s_step + 512);
   const uint32_t m = pred.needle_len;
-  const uint32_t nd_bytes = (m + 15u) & ~15u;
+  const uint32_t nd_bytes = IN ? kInTableBytes : ((m + 15u) & ~15u);  // IN lists: the needle table in place of the needle
   uint16_t* s_fail = reinterpret_cast<uint16_t*>(s_nd + nd_bytes);
   uint32_t* s_dict = reinterpret_cast<uint32_t*>(s_nd + nd_bytes + ((2u * m + 15u) & ~15u));
   uint16_t* s_cand = reinterpret_cast<uint16_t*>(s_dict + dict_words);
@@ -827,11 +927,11 @@ k_str_scan(ScanIo io, StrPredDesc pred, uint32_t stage_cap, uint32_t dict_words,
         v.resid = ref.blob + v.h->resid_off;
         v.fp = nullptr;
       }
-      str_scan_body<MODE>(v, w, pred, sm, s_sym, s_len, s_plan, s_nd, s_fail, s_dict, s_cand, s_M, s_step, dict_words,
+      str_scan_body<MODE, IN>(v, w, pred, sm, s_sym, s_len, s_plan, s_nd, s_fail, s_dict, s_cand, s_M, s_step, dict_words,
                           &sm->bar[1], parity, table_cache, t_start);
     } else {
       const StrView v = make_view(ref.blob, ref.blob);
-      str_scan_body<MODE>(v, w, pred, sm, s_sym, s_len, s_plan, s_nd, s_fail, s_dict, s_cand, s_M, s_step, dict_words,
+      str_scan_body<MODE, IN>(v, w, pred, sm, s_sym, s_len, s_plan, s_nd, s_fail, s_dict, s_cand, s_M, s_step, dict_words,
                           nullptr, 0, table_cache, t_start);
     }
     __syncthreads();  // the staged sections and the control area are reused by the next entry
@@ -1217,8 +1317,8 @@ k_str_like(ScanIo io, StrPredDesc pred_in, uint32_t dict_words, uint32_t n_entri
 
 static uint32_t str_like_smem(uint32_t dict_words) { return 8u * (16u + dict_words * 4u + kLikeCandCap * 2u); }
 
-static uint32_t str_scan_smem(uint32_t needle_len, uint32_t dict_words, uint32_t stage) {
-  const uint32_t nd = (needle_len + 15u) & ~15u;
+static uint32_t str_scan_smem(uint32_t needle_len, uint32_t dict_words, uint32_t stage, bool in_list) {
+  const uint32_t nd = in_list ? kInTableBytes : (needle_len + 15u) & ~15u;
   const uint32_t fl = (2u * needle_len + 15u) & ~15u;
   return kScanFixedSmem + kStrScanTables + nd + fl + dict_words * 4u + (((dict_words * 64u) + 127u) & ~127u) + 128u +
          stage;
@@ -1286,23 +1386,26 @@ cudaError_t launch_str_scan(int mode, uint32_t n_entries, const ScanIo& io, cons
     }
   }
   uint32_t stage = (max_head_bytes + 127u) & ~127u;
-  if (str_scan_smem(pred.needle_len, dict_words, stage) > 110u * 1024u) stage = 0;  // keep >= 2 CTAs per SM
-  const uint32_t smem = str_scan_smem(pred.needle_len, dict_words, stage);
+  const bool in_list = pred.op == LC_OP_IN || pred.op == LC_OP_NOT_IN;
+  if (str_scan_smem(pred.needle_len, dict_words, stage, in_list) > 110u * 1024u) stage = 0;  // keep >= 2 CTAs per SM
+  const uint32_t smem = str_scan_smem(pred.needle_len, dict_words, stage, in_list);
   if (smem > kMaxSmem) return cudaErrorInvalidValue;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k_str_scan<MODE_PRED>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_str_scan<MODE_REFINE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-    if (e != cudaSuccess) return e;
+    for (auto k : {k_str_scan<MODE_PRED, false>, k_str_scan<MODE_REFINE, false>, k_str_scan<MODE_PRED, true>,
+                   k_str_scan<MODE_REFINE, true>}) {
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+      if (e != cudaSuccess) return e;
+    }
     attr_set = true;
   }
   // consecutive entries per CTA (table reuse), as long as the grid still covers the GPU several times over
   uint32_t per_cta = n_entries / (148u * 4u * 3u);
   per_cta = per_cta < 1u ? 1u : (per_cta > 4u ? 4u : per_cta);
   const uint32_t grid = (n_entries + per_cta - 1u) / per_cta;
-  if (mode == MODE_PRED) k_str_scan<MODE_PRED><<<grid, 256, smem, s>>>(io, pred, stage, dict_words, n_entries, per_cta);
-  else k_str_scan<MODE_REFINE><<<grid, 256, smem, s>>>(io, pred, stage, dict_words, n_entries, per_cta);
+  auto kern = in_list ? (mode == MODE_PRED ? k_str_scan<MODE_PRED, true> : k_str_scan<MODE_REFINE, true>)
+                      : (mode == MODE_PRED ? k_str_scan<MODE_PRED, false> : k_str_scan<MODE_REFINE, false>);
+  kern<<<grid, 256, smem, s>>>(io, pred, stage, dict_words, n_entries, per_cta);
   return cudaGetLastError();
 }
 

@@ -52,11 +52,23 @@ struct ScanIo {
 // `col <op> literal` on an integer column, as it crossed the C ABI; lowered to the packed domain per entry
 // on the device (u = v - reference against a threshold, or a constant when the literal is outside the window).
 struct IntPredDesc {
-  int32_t op;        // lc_op EQ..GE
+  int32_t op;        // lc_op EQ..GE, or IN / NOT_IN (the values are then in an IntInList)
   int32_t lit_kind;  // LC_LIT_I64 / LC_LIT_U64 / kLitAboveAll
   int64_t lit_i;
   uint64_t lit_u;
 };
+// The values of `col [NOT] IN (list)` on an integer column: 64-bit patterns of the column's own domain, sorted in the
+// column's order (signed or unsigned) and without duplicates. Device memory (the host build of int_plan.cuh: host memory).
+struct IntInList {
+  const uint64_t* v;
+  uint32_t n;
+  uint32_t pad;
+};
+constexpr int32_t kOpIn = 10, kOpNotIn = 11;  // lc_op LC_OP_IN / LC_OP_NOT_IN
+constexpr uint32_t kInListMaxValues = 256;     // LC_IN_LIST_MAX_VALUES
+constexpr uint32_t kInListMaxBytes = 16384;    // LC_IN_LIST_MAX_BYTES
+// device buffer of one IN list: 8-byte integers, or int32 offsets[n + 1] + value bytes (+ padding)
+constexpr uint32_t kInListBlobCap = 4u * (kInListMaxValues + 1u) + kInListMaxBytes + 64u;
 constexpr int32_t kLitAboveAll = 7;  // decimal literal beyond u64: larger than every value of the column
 constexpr int32_t kLitSentinel = 8;  // squeezed (clamp) entries: "code == all ones of the entry's width", whatever the op says
 
@@ -78,13 +90,14 @@ struct alignas(16) IntPackWork {  // 96 bytes
 };
 static_assert(sizeof(IntPackWork) == 96, "IntPackWork must be 96 bytes");
 
+// `in` is read for IN / NOT_IN predicates only.
 cudaError_t launch_int_scan(int mode, uint32_t n_entries, const ScanIo& io, const IntPredDesc& pred,
-                            uint32_t max_blob_bytes, cudaStream_t s);
+                            uint32_t max_blob_bytes, cudaStream_t s, const IntInList& in = IntInList{});
 // Full-length integer predicates (REFINE, PRED over all rows) on lists whose entries all have fields of at most 32 bits:
 // register-resident FastLanes unpack, one warp per chunk (k_int_bits.cu). `io.counts`, if set, must be zeroed on the
 // stream before the launch; max_rows = rows of the longest entry of the list.
 cudaError_t launch_int_bits(int mode, uint32_t n_entries, const ScanIo& io, const IntPredDesc& pred, uint32_t max_rows,
-                            cudaStream_t s);
+                            cudaStream_t s, const IntInList& in = IntInList{});
 
 cudaError_t launch_int_minmax(const IntMinMaxWork* d_works, uint32_t n_works, cudaStream_t s);
 cudaError_t launch_int_pack(const IntPackWork* d_works, uint32_t n_works, cudaStream_t s);
@@ -169,6 +182,7 @@ enum StrPredKind : int32_t {
   SP_ORD = 3,       // prefix7 compare, ties decoded and compared in full (comparisons.rs:114-151,351-405)
   SP_ORD_EMPTY = 4, // needle suffix empty: decided on PrefixKey.len (comparisons.rs:371-381)
   SP_LIKE = 5,      // fingerprint gate + substring match on the encoded bytes (comparisons.rs:159-183,600-651)
+  SP_IN = 6,        // IN list: every needle planned like SP_EQ_*, looked up by PrefixKey, long ties compared in full
 };
 
 constexpr uint32_t kMaxNeedle = 1024;  // needle bytes staged into shared memory
@@ -188,6 +202,10 @@ struct alignas(16) StrPredDesc {
   // (512 x 16 bytes each, built per launch by k_like_steps) and each entry's index into them; nullptr = not prepared
   const void* like_steps;
   const uint32_t* entry_table;
+  // IN / NOT_IN: `needle` points at the list (int32 offsets[list_n + 1], then the value bytes; sorted, no duplicates)
+  // and needle_len is 0 (nothing is staged by the single-needle code)
+  uint32_t list_n;
+  uint32_t pad_list;
 };
 // One step table per distinct FSST symbol table of the list: d_tables[t] -> d_steps + t * 512 entries of 16 bytes.
 cudaError_t launch_like_steps(const uint64_t* d_tables, uint32_t n_tables, const StrPredDesc& pred, void* d_steps, cudaStream_t s);

@@ -441,6 +441,13 @@ int lc_squeezed_info(lc_ctx* ctx, lc_handle h, uint64_t out[6]) {
   return LC_OK;
 }
 
+// IN lists are planned on full entries only: a squeezed entry's codes would need a probe per list value.
+static int refuse_in_list_on_squeezed(const lc_predicate* pred) {
+  if (pred->op != LC_OP_IN && pred->op != LC_OP_NOT_IN) return LC_OK;
+  set_error("IN lists do not run on squeezed entries");
+  return LC_ERR_UNSUPPORTED_EXPR;
+}
+
 int lc_eval_predicate_many(lc_ctx* ctx, const lc_handle* handles, uint64_t n, const lc_predicate* pred,
                            const uint8_t* const* sel_bits, uint8_t* out_values, uint8_t* out_validity,
                            const uint64_t* out_byte_offsets, uint64_t* out_len, uint64_t* out_null_count,
@@ -459,6 +466,7 @@ int lc_eval_predicate_many(lc_ctx* ctx, const lc_handle* handles, uint64_t n, co
   PredOut po{out_values, out_validity, out_byte_offsets, out_len, out_null_count, out_true_count};
   bool any_squeezed = false;
   for (uint64_t i = 0; i < n && !any_squeezed; ++i) any_squeezed = es[i]->squeeze_kind != 0;
+  if (any_squeezed) LC_TRY(refuse_in_list_on_squeezed(pred));
   if (any_squeezed) return squeezed_eval_predicate_many(ctx, es, n, pred, sel_bits, po);  // probes + backing reads where needed
   return eval_predicate_batch(ctx, es, n, pred, sel_bits, po);
 }
@@ -481,6 +489,7 @@ int lc_eval_predicate(lc_ctx* ctx, lc_handle h, const lc_predicate* pred, const 
       set_error("lc_eval_predicate: NULL argument");
       return LC_ERR_INVALID;
     }
+    LC_TRY(refuse_in_list_on_squeezed(pred));
     Guard g(ctx);
     PredOut po{out_values, out_validity, &off0, out_len, out_null_count, nullptr};
     return squeezed_eval_predicate(ctx, e, pred, sel_bits, po);
@@ -854,6 +863,7 @@ int lc_scan_filter(lc_scan* scan, const lc_handle* handles, const lc_predicate* 
   Entry* const* es = nullptr;
   bool any_squeezed = false;
   LC_TRY(scan_entries_cached(scan, handles, &es, &any_squeezed));
+  if (any_squeezed) LC_TRY(refuse_in_list_on_squeezed(pred));
   if (any_squeezed) LC_TRY(scan_filter_squeezed(scan, es, pred));
   else LC_TRY(refine_batch(ctx, es, scan->n, pred, scan->d_sel, scan->d_word_off, scan->all_rows, scan->d_counts));
   scan->all_rows = false;

@@ -50,10 +50,12 @@ struct BooleanBuffer {
 // A validated predicate (LiquidExpr, src/core/src/cache/liquid_expr.rs:33-44) already lowered to (op, literal).
 struct LiquidExpr {
   lc_predicate pred{};
-  std::string bytes;  // owns the literal for byte-like columns
+  std::string bytes;  // owns the literal for byte-like columns, and the encoded values of an IN list
   // the native form with the literal pointer taken from THIS object's bytes (copies and moves of a LiquidExpr stay valid)
   const lc_predicate* native() {
-    if (pred.lit_kind == LC_LIT_BYTES) {
+    if (pred.op == LC_OP_IN || pred.op == LC_OP_NOT_IN) {
+      pred.lit_bytes = reinterpret_cast<const uint8_t*>(bytes.data());  // lit_len stays the number of values
+    } else if (pred.lit_kind == LC_LIT_BYTES) {
       pred.lit_bytes = reinterpret_cast<const uint8_t*>(bytes.data());
       pred.lit_len = bytes.size();
     }
@@ -101,6 +103,40 @@ struct LiquidExpr {
   }
   static LiquidExpr like(std::string pattern, bool negated = false) {
     return compare_bytes(negated ? LC_OP_NOT_LIKE : LC_OP_LIKE, std::move(pattern));
+  }
+  // `col [NOT] IN (values)` (InListExpr; the reference's LiquidExpr does not admit it): integer / date / timestamp columns
+  static LiquidExpr in_list_i64(const std::vector<int64_t>& values, bool negated = false) {
+    return in_list_words(LC_LIT_I64, values.data(), values.size(), negated);
+  }
+  static LiquidExpr in_list_u64(const std::vector<uint64_t>& values, bool negated = false) {
+    return in_list_words(LC_LIT_U64, values.data(), values.size(), negated);
+  }
+  // byte-like columns: the values in Arrow's Utf8 layout, int32 offsets[n + 1] then the bytes
+  static LiquidExpr in_list_bytes(const std::vector<std::string>& values, bool negated = false) {
+    LiquidExpr e;
+    e.pred.op = negated ? LC_OP_NOT_IN : LC_OP_IN;
+    e.pred.lit_kind = LC_LIT_BYTES;
+    e.pred.lit_len = values.size();
+    int32_t off = 0;
+    e.bytes.append(reinterpret_cast<const char*>(&off), 4);
+    for (const std::string& v : values) {
+      off += static_cast<int32_t>(v.size());
+      e.bytes.append(reinterpret_cast<const char*>(&off), 4);
+    }
+    for (const std::string& v : values) e.bytes += v;
+    e.native();
+    return e;
+  }
+
+ private:
+  static LiquidExpr in_list_words(int32_t kind, const void* words, size_t n, bool negated) {
+    LiquidExpr e;
+    e.pred.op = negated ? LC_OP_NOT_IN : LC_OP_IN;
+    e.pred.lit_kind = kind;
+    e.pred.lit_len = n;
+    e.bytes.assign(static_cast<const char*>(words), n * 8);  // little-endian hosts: the words as they are in memory
+    e.native();
+    return e;
   }
 };
 

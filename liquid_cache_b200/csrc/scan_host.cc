@@ -242,11 +242,67 @@ struct StrLaunch {
   uint32_t m = 0;
 };
 
+static bool is_in_list(const lc_predicate* pred) { return pred->op == LC_OP_IN || pred->op == LC_OP_NOT_IN; }
+
+// `col [NOT] IN (list)` on byte-view entries: the list checked (Arrow Utf8 layout), sorted and deduplicated, and laid out
+// again the same way — int32 offsets[k + 1], then the bytes — as the buffer k_str_scan plans its needles from.
+static int prepare_str_in_list(const lc_predicate* pred, StrLaunch* L) {
+  if (pred->lit_kind != LC_LIT_BYTES) {
+    set_error("IN list on a byte-view column needs LC_LIT_BYTES values");
+    return LC_ERR_UNSUPPORTED_EXPR;
+  }
+  const uint64_t n = pred->lit_len;
+  if (n > kInListMaxValues) {
+    set_error("IN list of %llu values: at most %u run on the device", (unsigned long long)n, kInListMaxValues);
+    return LC_ERR_UNSUPPORTED_EXPR;
+  }
+  if (!pred->lit_bytes) {
+    set_error("IN list without its offsets");
+    return LC_ERR_INVALID;
+  }
+  std::vector<int32_t> off(n + 1);
+  std::memcpy(off.data(), pred->lit_bytes, (n + 1) * 4);
+  if (off[0] != 0) {
+    set_error("IN list: offsets[0] is %d, not 0", off[0]);
+    return LC_ERR_INVALID;
+  }
+  for (uint64_t i = 0; i < n; ++i)
+    if (off[i + 1] < off[i]) {
+      set_error("IN list: offsets decrease at value %llu", (unsigned long long)i);
+      return LC_ERR_INVALID;
+    }
+  if (static_cast<uint64_t>(off[n]) > kInListMaxBytes) {
+    set_error("IN list of %d value bytes: at most %u run on the device", off[n], kInListMaxBytes);
+    return LC_ERR_UNSUPPORTED_EXPR;
+  }
+  const char* bytes = reinterpret_cast<const char*>(pred->lit_bytes) + (n + 1) * 4;
+  std::vector<std::string> vals;
+  vals.reserve(n);
+  for (uint64_t i = 0; i < n; ++i) vals.emplace_back(bytes + off[i], static_cast<size_t>(off[i + 1] - off[i]));
+  std::sort(vals.begin(), vals.end());
+  vals.erase(std::unique(vals.begin(), vals.end()), vals.end());
+  const uint32_t k = static_cast<uint32_t>(vals.size());
+  L->needle_blob.assign(4u * (k + 1u), 0);
+  int32_t o = 0;
+  for (uint32_t i = 0; i <= k; ++i) {
+    std::memcpy(L->needle_blob.data() + 4u * i, &o, 4);
+    if (i < k) o += static_cast<int32_t>(vals[i].size());
+  }
+  for (const std::string& v : vals) L->needle_blob.insert(L->needle_blob.end(), v.begin(), v.end());
+  L->needle_blob.resize((L->needle_blob.size() + 3u) & ~size_t(3), 0);
+  L->desc.list_n = k;
+  L->desc.needle_len = 0;
+  L->needle = nullptr;
+  L->m = 0;
+  return LC_OK;
+}
+
 static int prepare_str_pred(const lc_predicate* pred, StrLaunch* L) {
   std::memset(&L->desc, 0, sizeof(L->desc));
   L->desc.op = pred->op;
   const int op = pred->op;
   if (op == LC_OP_CONST_TRUE || op == LC_OP_CONST_FALSE) return LC_OK;
+  if (is_in_list(pred)) return prepare_str_in_list(pred, L);
   if (pred->lit_kind != LC_LIT_BYTES || (!pred->lit_bytes && pred->lit_len)) {
     set_error("byte-view column needs a bytes literal");
     return LC_ERR_UNSUPPORTED_EXPR;
@@ -479,6 +535,57 @@ static int get_ref_list(lc_ctx* ctx, Entry* const* entries, uint64_t n, const Re
   }
   rc.lists.push_back(nl);
   *out = &rc.lists.back();
+  return LC_OK;
+}
+
+// `col [NOT] IN (list)` on integer / date / timestamp entries: the values in the column's domain, sorted in the column's
+// order (signed or unsigned, the same for every entry of the list) without duplicates, as 8-byte words ready to upload.
+// Values no entry can hold (negative on an unsigned column, above i64::MAX on a signed one) are dropped.
+static int make_int_in_list(const lc_predicate* pred, Entry* const* entries, uint64_t n, IntPredDesc* out,
+                            std::vector<uint8_t>* blob) {
+  if (entries[0]->liquid_type != LC_LIQUID_INTEGER) {
+    set_error("IN lists run on integer, date, timestamp and byte-view columns only");
+    return LC_ERR_UNSUPPORTED_EXPR;
+  }
+  if (pred->lit_kind != LC_LIT_I64 && pred->lit_kind != LC_LIT_U64) {
+    set_error("IN list on an integer column needs LC_LIT_I64 or LC_LIT_U64 values");
+    return LC_ERR_UNSUPPORTED_EXPR;
+  }
+  if (pred->lit_len > kInListMaxValues) {
+    set_error("IN list of %llu values: at most %u run on the device", (unsigned long long)pred->lit_len, kInListMaxValues);
+    return LC_ERR_UNSUPPORTED_EXPR;
+  }
+  if (pred->lit_len && !pred->lit_bytes) {
+    set_error("IN list without its values");
+    return LC_ERR_INVALID;
+  }
+  const bool is_signed = entries[0]->ih.is_signed != 0;
+  for (uint64_t i = 1; i < n; ++i)
+    if ((entries[i]->ih.is_signed != 0) != is_signed) {
+      set_error("IN list over signed and unsigned integer entries in one call");
+      return LC_ERR_INVALID;
+    }
+  std::vector<uint64_t> v;
+  v.reserve(pred->lit_len);
+  for (uint64_t i = 0; i < pred->lit_len; ++i) {
+    uint64_t x;
+    std::memcpy(&x, pred->lit_bytes + 8 * i, 8);
+    const bool neg_i64 = pred->lit_kind == LC_LIT_I64 && static_cast<int64_t>(x) < 0;
+    const bool big_u64 = pred->lit_kind == LC_LIT_U64 && x > 0x7fffffffffffffffull;
+    if ((is_signed && big_u64) || (!is_signed && neg_i64)) continue;
+    v.push_back(x);
+  }
+  if (is_signed)
+    std::sort(v.begin(), v.end(), [](uint64_t a, uint64_t b) { return static_cast<int64_t>(a) < static_cast<int64_t>(b); });
+  else
+    std::sort(v.begin(), v.end());
+  v.erase(std::unique(v.begin(), v.end()), v.end());
+  blob->resize(v.size() * 8);
+  if (!v.empty()) std::memcpy(blob->data(), v.data(), v.size() * 8);
+  out->op = pred->op;
+  out->lit_kind = is_signed ? LC_LIT_I64 : LC_LIT_U64;
+  out->lit_i = 0;
+  out->lit_u = 0;
   return LC_OK;
 }
 
@@ -789,12 +896,15 @@ int eval_predicate_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const l
   LC_TRY(plan_selection(ctx, rl->rows->data(), n, sel_bits, &sp));
   StrLaunch sl;
   IntPredDesc ip{};
-  if (is_int) LC_TRY(make_int_pred(pred, entries[0], &ip));
+  std::vector<uint8_t> int_list;  // IN lists on integer entries
+  if (is_int && is_in_list(pred)) LC_TRY(make_int_in_list(pred, entries, n, &ip, &int_list));
+  else if (is_int) LC_TRY(make_int_pred(pred, entries[0], &ip));
   else LC_TRY(prepare_str_pred(pred, &sl));
+  const std::vector<uint8_t>& needle_blob = is_int ? int_list : sl.needle_blob;
 
-  // upload: sel_off[n] | out_off[n] | needle | selection words ; download: counts[2n] | mask words | validity words
+  // upload: sel_off[n] | out_off[n] | needle (or IN list) | selection words ; download: counts[2n] | mask words | validity words
   const uint64_t up_offs = round_up(n * 16, 256);
-  const uint64_t up_needle = is_int ? 0 : round_up(sl.needle_blob.size(), 256);
+  const uint64_t up_needle = round_up(needle_blob.size(), 256);
   const uint64_t up_sel = round_up(sp.sel_words * 4, 256);
   const uint64_t up_total = up_offs + up_needle + up_sel;
   const bool any_nulls = rl->any_nulls;
@@ -845,7 +955,8 @@ int eval_predicate_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const l
     h_sel_off[i] = sp.bits[i] ? sp.word_off[i] : kNoSel;
     h_out_off[i] = out_word_off[i];
   }
-  if (!is_int) std::memcpy(h_up + up_offs, sl.needle_blob.data(), sl.needle_blob.size());
+  if (!needle_blob.empty()) std::memcpy(h_up + up_offs, needle_blob.data(), needle_blob.size());
+  const IntInList in_list{reinterpret_cast<const uint64_t*>(d_up + up_offs), static_cast<uint32_t>(int_list.size() / 8), 0};
   ScanIo io{};
   io.refs = rl->d_refs;
   io.sel_base = sp.sel_words ? reinterpret_cast<const uint32_t*>(d_up + up_offs + up_needle) : nullptr;
@@ -913,9 +1024,9 @@ int eval_predicate_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const l
     ioc.valid_off += c0;
     ioc.counts += c0 * io.counts_stride;
     if (is_int && int_bits) {
-      LC_CUDA_OK(launch_int_bits(MODE_PRED, static_cast<uint32_t>(c1 - c0), ioc, ip, rl->max_rows, s));
+      LC_CUDA_OK(launch_int_bits(MODE_PRED, static_cast<uint32_t>(c1 - c0), ioc, ip, rl->max_rows, s, in_list));
     } else if (is_int) {
-      LC_CUDA_OK(launch_int_scan(MODE_PRED, static_cast<uint32_t>(c1 - c0), ioc, ip, rl->max_blob, s));
+      LC_CUDA_OK(launch_int_scan(MODE_PRED, static_cast<uint32_t>(c1 - c0), ioc, ip, rl->max_blob, s, in_list));
     } else {
       StrPredDesc dc = sl.desc;
       if (dc.entry_table) dc.entry_table += c0;
@@ -1084,8 +1195,33 @@ int refine_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const lc_predic
   const bool is_int = is_int_blob(entries[0]->liquid_type);
   StrLaunch sl;
   IntPredDesc ip{};
-  if (is_int) LC_TRY(make_int_pred(pred, entries[0], &ip));
+  std::vector<uint8_t> int_list;  // IN lists on integer entries
+  if (is_int && is_in_list(pred)) LC_TRY(make_int_in_list(pred, entries, n, &ip, &int_list));
+  else if (is_int) LC_TRY(make_int_pred(pred, entries[0], &ip));
   else LC_TRY(prepare_str_pred(pred, &sl));
+  cudaStream_t s = ctx->L()->stream;
+  // The needle (or IN list) is the only thing that travels: a few bytes from pageable memory (the runtime stages such
+  // copies before returning) into a small buffer the context keeps for this purpose.
+  const std::vector<uint8_t>& needle_blob = is_int ? int_list : sl.needle_blob;
+  uint8_t* d_nd = nullptr;
+  if (!needle_blob.empty()) {
+    if (!ctx->L()->d_needle) {
+      if (cudaMalloc(reinterpret_cast<void**>(&ctx->L()->d_needle), std::max<size_t>(2 * (kMaxNeedle + 16) * 2, kInListBlobCap)) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("cudaMalloc for the needle buffer failed");
+        return LC_ERR_OOM;
+      }
+    }
+    d_nd = ctx->L()->d_needle;
+    const std::string needle_key(reinterpret_cast<const char*>(needle_blob.data()), needle_blob.size());
+    if (ctx->L()->needle_in_buffer != needle_key || ctx->L()->needle_stream != s) {  // the buffer already holds it otherwise
+      LC_CUDA_OK(cudaMemcpyAsync(d_nd, needle_blob.data(), needle_blob.size(), cudaMemcpyHostToDevice, s));
+      ctx->h2d_bytes += needle_blob.size();
+      ctx->L()->needle_in_buffer = needle_key;
+      ctx->L()->needle_stream = s;
+    }
+  }
+  const IntInList in_list{reinterpret_cast<const uint64_t*>(d_nd), static_cast<uint32_t>(int_list.size() / 8), 0};
   ScanIo io{};
   io.refs = rl->d_refs;
   io.sel_base = all_rows ? nullptr : d_sel_base;
@@ -1096,30 +1232,13 @@ int refine_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const lc_predic
   io.valid_off = nullptr;
   io.counts = d_counts;
   io.counts_stride = 2;
-  cudaStream_t s = ctx->L()->stream;
   if (is_int) {
     if (rl->int_bits_ok && d_counts) LC_CUDA_OK(cudaMemsetAsync(d_counts, 0, n * 8, s));  // k_int_bits adds per chunk
     if (ctx->L()->timing_on) cudaEventRecord(ctx->L()->ev_a, s);
-    if (rl->int_bits_ok) LC_CUDA_OK(launch_int_bits(MODE_REFINE, static_cast<uint32_t>(n), io, ip, rl->max_rows, s));
-    else LC_CUDA_OK(launch_int_scan(MODE_REFINE, static_cast<uint32_t>(n), io, ip, rl->max_blob, s));
+    if (rl->int_bits_ok) LC_CUDA_OK(launch_int_bits(MODE_REFINE, static_cast<uint32_t>(n), io, ip, rl->max_rows, s, in_list));
+    else LC_CUDA_OK(launch_int_scan(MODE_REFINE, static_cast<uint32_t>(n), io, ip, rl->max_blob, s, in_list));
   } else {
-    // the needle is the only thing that travels: a few bytes from pageable memory (the runtime stages such
-    // copies before returning) into a small buffer the context keeps for this purpose
-    if (!ctx->L()->d_needle) {
-      if (cudaMalloc(reinterpret_cast<void**>(&ctx->L()->d_needle), 2 * (kMaxNeedle + 16) * 2) != cudaSuccess) {
-        cudaGetLastError();
-        set_error("cudaMalloc for the needle buffer failed");
-        return LC_ERR_OOM;
-      }
-    }
-    uint8_t* d_nd = ctx->L()->d_needle;
     const std::string needle_key(reinterpret_cast<const char*>(sl.needle_blob.data()), sl.needle_blob.size());
-    if (ctx->L()->needle_in_buffer != needle_key || ctx->L()->needle_stream != s) {  // the buffer already holds it otherwise
-      LC_CUDA_OK(cudaMemcpyAsync(d_nd, sl.needle_blob.data(), sl.needle_blob.size(), cudaMemcpyHostToDevice, s));
-      ctx->h2d_bytes += sl.needle_blob.size();
-      ctx->L()->needle_in_buffer = needle_key;
-      ctx->L()->needle_stream = s;
-    }
     sl.desc.needle = d_nd;
     sl.desc.prof = ctx->prof_on ? ctx->d_prof : nullptr;
     const bool like = (pred->op == LC_OP_LIKE || pred->op == LC_OP_NOT_LIKE);

@@ -49,6 +49,16 @@ class LikeExpr:
 
 
 @dataclass(frozen=True)
+class InListExpr:
+    """`InListExpr { expr, list, negated }`: `expr [NOT] IN (list)`. The reference's LiquidExpr does not admit it
+    (`try_new` returns None); `LiquidExpr.new_unchecked(InListExpr(...))` lowers it to LC_OP_IN / LC_OP_NOT_IN."""
+
+    expr: Any
+    list: tuple
+    negated: bool = False
+
+
+@dataclass(frozen=True)
 class CastExpr:
     expr: Any
     cast_type: Optional[pa.DataType] = None
@@ -240,7 +250,60 @@ class LiquidExpr:
                 p.lit_kind = N.LIT_U64
                 p.lit_u64 = v
             return p
+        if isinstance(e, InListExpr):
+            return _lower_in_list(e, column_type)
         raise N.UnsupportedExpr(N.LC_ERR_UNSUPPORTED_EXPR, f"expression shape {type(e).__name__}")
+
+
+def _lower_in_list(e: "InListExpr", column_type: pa.DataType) -> N.Predicate:
+    """`col [NOT] IN (v1, ..., vn)` -> LC_OP_IN / LC_OP_NOT_IN. The column side follows the rules of a comparison; the
+    values are n little-endian 8-byte integers (LC_LIT_I64, or LC_LIT_U64 when one exceeds i64) or, on byte-like columns,
+    Arrow's Utf8 layout (int32 offsets[n + 1], then the bytes). Null or non-literal elements are refused."""
+    def refuse(why):
+        raise N.UnsupportedExpr(N.LC_ERR_UNSUPPORTED_EXPR, why)
+
+    p = N.Predicate()
+    p.op = N.OP_NOT_IN if e.negated else N.OP_IN
+    items = list(e.list)
+    for it in items:
+        if not isinstance(it, Literal) or it.value is None:
+            refuse("IN list element is not a non-null literal")
+    if is_byte_like(column_type):
+        if not _is_column_like(e.expr):
+            refuse("IN list: column side is not column-like")
+        needles = [_bytes_needle(it) for it in items]
+        if any(nd is None for nd in needles):
+            refuse("IN list element is not bytes-like")
+        offs = _np.zeros(len(needles) + 1, dtype="<i4")
+        offs[1:] = _np.cumsum([len(nd) for nd in needles], dtype=_np.int64) if needles else []
+        _set_bytes(p, offs.tobytes() + b"".join(needles))
+        p.lit_len = len(needles)
+        return p
+    if pa.types.is_floating(column_type) or pa.types.is_decimal(column_type):
+        refuse("IN list on a float / decimal column")
+    if not _cast_chain_is_integer_identity(e.expr, column_type):
+        refuse("IN list: column side is not an integer-preserving cast chain")
+    outer = _outermost_type(e.expr, column_type)
+    vals = []
+    for it in items:
+        v = _int_literal(it, outer)
+        if v is None:
+            refuse("IN list element is not an integer/date/timestamp")
+        if not (-(1 << 63) <= v <= 0xFFFFFFFFFFFFFFFF):
+            refuse("IN list element out of the 64-bit range")
+        vals.append(v)
+    if any(v > 0x7FFFFFFFFFFFFFFF for v in vals):
+        if any(v < 0 for v in vals):
+            refuse("IN list mixes negative values with values above i64")
+        p.lit_kind = N.LIT_U64
+        raw = _np.array(vals, dtype="<u8").tobytes()
+    else:
+        p.lit_kind = N.LIT_I64
+        raw = _np.array(vals, dtype="<i8").tobytes()
+    p._keepalive = raw
+    p.lit_bytes = raw
+    p.lit_len = len(vals)
+    return p
 
 
 def _set_bytes(p: N.Predicate, needle: bytes) -> None:
