@@ -355,6 +355,7 @@ int lc_cache_eval_predicate(lc_ctx* ctx, uint64_t entry_id, const lc_predicate* 
  *
  *   lc_scan_begin(n_batches, rows[i])            running selection := all rows
  *   lc_scan_filter(scan, handles[i], pred)       selection := and_then(selection, eval(handles[i]))
+ *   lc_scan_filter_or(scan, terms, ...)          selection &= OR of AND groups of such predicates
  *   lc_scan_counts(scan, counts[i])              popcount(selection_i)  (one D2H of n u32)
  *   lc_scan_selection(scan, i, bits)             copy selection of batch i to host
  *   lc_scan_read(scan, handles[i], out)          concatenated get().with_selection(selection_i)
@@ -373,6 +374,21 @@ int lc_scan_selection_layout(lc_scan* scan, uint64_t* word_offsets, uint64_t* to
 int lc_scan_store_selections(lc_scan* scan, uint32_t* out_words, uint64_t n_words);
 int lc_scan_load_selections(lc_scan* scan, const uint32_t* words, uint64_t n_words);
 int lc_scan_filter(lc_scan* scan, const lc_handle* handles, const lc_predicate* pred);
+/* A disjunction over columns as ONE conjunct of the scan: CachedRowGroup::evaluate_selection_with_predicate's
+ * multi-column OR (src/datafusion/src/cache/mod.rs:111-150: every leaf evaluated under the same selection, the masks
+ * joined with or_kleene), generalised to an OR of AND groups:
+ *   selection := selection AND OR_d ( AND_{t in d} (valid_t AND preds[t]) )
+ *   handles[t]  n_batches handles of term t's column, in the scan's batch order (several terms may name one column)
+ *   preds[t]    anything lc_scan_filter accepts on that column
+ *   group[t]    disjunct of term t: non-decreasing, starting at 0, without gaps; NULL = every term its own disjunct
+ * A null term is false, which is exact: a DNF row is TRUE under Kleene logic exactly when some disjunct has every term
+ * TRUE, and the reader turns null into false. Bad arguments (n_terms == 0, NULL pointers, a malformed group, handles whose
+ * row counts differ from the scan's) return LC_ERR_INVALID; a term lc_scan_filter would refuse returns its refusal
+ * (LC_ERR_UNSUPPORTED_EXPR). Either way the running selection and its counts are left as they were. Cost: the kernels of
+ * every term as lc_scan_filter would launch them, plus one merge kernel per disjunct; nothing crosses PCIe that
+ * lc_scan_filter would not move for the same terms. */
+int lc_scan_filter_or(lc_scan* scan, uint64_t n_terms, const lc_handle* const* handles, const lc_predicate* preds,
+                      const uint32_t* group);
 int lc_scan_counts(lc_scan* scan, uint64_t* out_counts, uint64_t* out_total);
 int lc_scan_selection(lc_scan* scan, uint64_t batch, uint8_t* out_bits);
 int lc_scan_read(lc_scan* scan, const lc_handle* handles, struct ArrowSchema* out_schema,

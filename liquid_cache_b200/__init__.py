@@ -8,10 +8,11 @@ from . import _native
 from .cache import (EntryID, EvaluatePredicate, Get, GpuLiquidArray, Insert, LiquidCache, LiquidCacheBuilder, Scan,
                     parquet_array_id, selection_bits)
 from .expr import (BinaryExpr, CacheExpression, CastColumnExpr, CastExpr, Column, DynamicFilterPhysicalExpr, InListExpr,
-                   LikeExpr, LiquidExpr, Literal, ScalarFunctionExpr, TryCastExpr)
+                   LikeExpr, LiquidExpr, Literal, ScalarFunctionExpr, TryCastExpr, split_disjunction)
 
 __all__ = [
     "EntryID", "EvaluatePredicate", "Get", "GpuLiquidArray", "Insert", "LiquidCache", "LiquidCacheBuilder", "Scan",
     "parquet_array_id", "selection_bits", "BinaryExpr", "CacheExpression", "CastColumnExpr", "CastExpr", "Column",
     "DynamicFilterPhysicalExpr", "InListExpr", "LikeExpr", "LiquidExpr", "Literal", "ScalarFunctionExpr", "TryCastExpr",
+    "split_disjunction",
 ]

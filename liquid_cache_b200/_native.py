@@ -150,6 +150,7 @@ def lib() -> C.CDLL:
     l.lc_ctx_profile_counters.argtypes = [vp, C.c_int, vp]
     l.lc_scan_set_selection.argtypes = [vp, u64, vp, u64]
     l.lc_scan_filter.argtypes = [vp, vp, C.POINTER(Predicate)]
+    l.lc_scan_filter_or.argtypes = [vp, u64, vp, C.POINTER(Predicate), vp]
     l.lc_scan_counts.argtypes = [vp, vp, u64p]
     l.lc_scan_selection.argtypes = [vp, u64, vp]
     l.lc_scan_read.argtypes = [vp, vp, vp, vp]

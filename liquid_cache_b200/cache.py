@@ -614,6 +614,46 @@ class LiquidCache:
         return Scan(self, rows_per_batch)
 
 
+def or_terms(disjuncts) -> tuple[list, list, list]:
+    """[[(handles, LiquidExpr, column_type), ...], ...] -> (handles per term, lowered predicates, disjunct per term), the
+    arguments of `Scan.filter_or_native`. Raises UnsupportedExpr for a leaf `LiquidExpr.to_native` cannot lower."""
+    if not disjuncts or any(len(d) == 0 for d in disjuncts):
+        raise ValueError("filter_or: needs at least one disjunct, and at least one term in each")
+    handles, preds, group = [], [], []
+    for g, d in enumerate(disjuncts):
+        for h, expr, typ in d:
+            handles.append(h)
+            preds.append(expr.to_native(typ))
+            group.append(g)
+    return handles, preds, group
+
+
+def pack_or_terms(handles_per_term, preds, group, n_batches: int):
+    """Checks the arguments of lc_scan_filter_or and packs them for ctypes: (pointer array of the handle lists, the arrays
+    it points into, Predicate array, group array or None)."""
+    n = len(preds)
+    if n == 0:
+        raise ValueError("filter_or: no terms")
+    if len(handles_per_term) != n:
+        raise ValueError(f"filter_or: {len(handles_per_term)} handle lists for {n} predicates")
+    keep = [np.ascontiguousarray(h, dtype=np.uint64) for h in handles_per_term]
+    for t, h in enumerate(keep):
+        if h.ndim != 1 or len(h) != n_batches:
+            raise ValueError(f"filter_or: term {t} has {h.size} handles, the scan has {n_batches} batches")
+    g_arr = None
+    if group is not None:
+        g = [int(x) for x in group]
+        if len(g) != n:
+            raise ValueError(f"filter_or: {len(g)} group indices for {n} terms")
+        if g[0] != 0 or any(b - a not in (0, 1) for a, b in zip(g, g[1:])):
+            raise ValueError("filter_or: group must start at 0 and be non-decreasing without gaps")
+        g_arr = (C.c_uint32 * n)(*g)
+    h_ptrs = (C.c_void_p * n)(*[h.ctypes.data for h in keep])
+    p_arr = (N.Predicate * n)(*preds)
+    keep.append(list(preds))  # the literal bytes the copied structs point at
+    return h_ptrs, keep, p_arr, g_arr
+
+
 class Scan:
     """The per-batch loop of `LiquidCacheReader::build_predicate_filter` + `read_from_cache`
     (/root/reference/src/datafusion/src/reader/runtime/liquid_cache_reader.rs:297-391) for many batches at
@@ -674,6 +714,18 @@ class Scan:
     def filter_native(self, handles: np.ndarray, pred: N.Predicate) -> None:
         handles = np.ascontiguousarray(handles, dtype=np.uint64)
         N.check(N.lib().lc_scan_filter(self._scan, handles.ctypes.data, C.byref(pred)))
+
+    def filter_or(self, disjuncts) -> None:
+        """One conjunct that is an OR of AND groups: `disjuncts` = [[(handles, LiquidExpr, column_type), ...], ...];
+        selection &= OR over the groups of (AND over the group's terms). Every leaf is lowered like `filter` lowers it."""
+        self.filter_or_native(*or_terms(disjuncts))
+
+    def filter_or_native(self, handles_per_term, preds, group=None) -> None:
+        """lc_scan_filter_or: `handles_per_term[t]` the batch handles of term t, `preds[t]` its lowered predicate,
+        `group[t]` its disjunct (non-decreasing from 0, no gaps; None = every term its own disjunct)."""
+        h_ptrs, keep, p_arr, g_arr = pack_or_terms(handles_per_term, preds, group, len(self._rows))
+        N.check(N.lib().lc_scan_filter_or(self._scan, len(preds), h_ptrs, p_arr, g_arr))
+        del keep
 
     def counts(self) -> tuple[np.ndarray, int]:
         out = np.zeros(len(self._rows), dtype=np.uint64)

@@ -232,4 +232,61 @@ cudaError_t launch_and_then(const uint32_t* d_left, uint32_t left_bits, const ui
   return cudaGetLastError();
 }
 
+// lc_scan_filter_or: the merge that closes one disjunct. `term` holds the rows of the disjunct's remainder that passed
+// every one of its terms, `acc` the rows accepted by the disjuncts before it, `sel` the running selection (sel_all: every
+// row). Not last: acc := acc | term, term := sel & ~acc (where the next disjunct starts). Last: sel := acc | term and
+// counts[2i] its popcount (counts[2i + 1] = 0, the stride-2 layout of the REFINE kernels). One warp per batch, 16-byte
+// words; bits at or past rows[i], and the padding up to the batch's 4-word boundary, are written as zero whatever the
+// refine kernels left there.
+__global__ void __launch_bounds__(256) k_sel_or(uint32_t* __restrict__ sel, uint32_t sel_all, uint32_t* __restrict__ term,
+                                                uint32_t* __restrict__ acc, const uint64_t* __restrict__ word_off,
+                                                const uint32_t* __restrict__ rows, uint32_t n, uint32_t first, uint32_t last,
+                                                uint32_t* __restrict__ counts) {
+  const uint32_t b = blockIdx.x * 8u + (threadIdx.x >> 5);
+  if (b >= n) return;
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t r = rows[b];
+  const uint32_t full = r >> 5, tail = r & 31u;
+  const uint32_t vecs = (((r + 31u) >> 5) + 3u) >> 2;
+  const uint64_t base = word_off[b] >> 2;  // batches start on a 4-word boundary
+  uint4* T = reinterpret_cast<uint4*>(term) + base;
+  uint4* A = reinterpret_cast<uint4*>(acc) + base;
+  uint4* S = reinterpret_cast<uint4*>(sel) + base;
+  uint32_t survivors = 0;
+  for (uint32_t v = lane; v < vecs; v += 32u) {
+    uint32_t valid[4];
+#pragma unroll
+    for (uint32_t j = 0; j < 4; ++j) {
+      const uint32_t w = v * 4u + j;
+      valid[j] = w < full ? kFullMask : (w == full && tail ? (1u << tail) - 1u : 0u);
+    }
+    const uint4 t = T[v];
+    const uint4 a = first ? make_uint4(0u, 0u, 0u, 0u) : A[v];
+    const uint4 u = make_uint4((a.x | t.x) & valid[0], (a.y | t.y) & valid[1], (a.z | t.z) & valid[2], (a.w | t.w) & valid[3]);
+    if (last) {
+      S[v] = u;
+      survivors += __popc(u.x) + __popc(u.y) + __popc(u.z) + __popc(u.w);
+    } else {
+      A[v] = u;
+      const uint4 s = sel_all ? make_uint4(valid[0], valid[1], valid[2], valid[3]) : S[v];
+      T[v] = make_uint4(s.x & ~u.x & valid[0], s.y & ~u.y & valid[1], s.z & ~u.z & valid[2], s.w & ~u.w & valid[3]);
+    }
+  }
+  if (last) {
+    survivors = warp_sum(survivors);
+    if (lane == 0) {
+      counts[2u * b] = survivors;
+      counts[2u * b + 1u] = 0u;
+    }
+  }
+}
+
+cudaError_t launch_sel_or(uint32_t* d_sel, bool sel_all, uint32_t* d_term, uint32_t* d_acc, const uint64_t* d_word_off,
+                          const uint32_t* d_rows, uint32_t n, bool first, bool last, uint32_t* d_counts, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  k_sel_or<<<(n + 7u) / 8u, 256, 0, s>>>(d_sel, sel_all ? 1u : 0u, d_term, d_acc, d_word_off, d_rows, n, first ? 1u : 0u,
+                                         last ? 1u : 0u, d_counts);
+  return cudaGetLastError();
+}
+
 }  // namespace lc

@@ -355,5 +355,11 @@ cudaError_t launch_fixed_from_var(const int32_t* d_offsets, uint32_t total_bytes
                                   uint64_t rows, uint32_t width, void* d_out, cudaStream_t s);
 cudaError_t launch_and_then(const uint32_t* d_left, uint32_t left_bits, const uint32_t* d_right, uint32_t* d_out,
                             cudaStream_t s);
+// lc_scan_filter_or, end of one disjunct over the scan's selection layout (batch i: word_off[i], rows[i] bits, padded to 4
+// words). Not last: acc := (first ? term : acc | term), term := sel & ~acc. Last: sel := (first ? term : acc | term),
+// counts[2i] = its popcount, counts[2i + 1] = 0. sel_all: the running selection is every row (sel is only written when
+// last). Tail bits and padding come out zero.
+cudaError_t launch_sel_or(uint32_t* d_sel, bool sel_all, uint32_t* d_term, uint32_t* d_acc, const uint64_t* d_word_off,
+                          const uint32_t* d_rows, uint32_t n, bool first, bool last, uint32_t* d_counts, cudaStream_t s);
 
 }  // namespace lc

@@ -83,6 +83,12 @@ struct lc_scan {
   uint32_t* d_probe = nullptr;
   uint32_t* d_save = nullptr;
   uint32_t* d_pcounts = nullptr;
+  // lc_scan_filter_or only, allocated on first use: the term buffer T and the accumulator A (selection-sized), counts the
+  // term launches write (nobody reads them) and the batch row counts k_sel_or masks the tails with
+  uint32_t* d_term = nullptr;
+  uint32_t* d_acc = nullptr;
+  uint32_t* d_tcounts = nullptr;
+  uint32_t* d_rows = nullptr;
   bool all_rows = true;       // no filter applied yet
   bool counts_on_device = false;
   bool counts_cached = false;
@@ -773,7 +779,11 @@ int lc_scan_set_selection(lc_scan* scan, uint64_t batch, const uint8_t* sel_bits
 //           codes cannot decide (hybrid_primitive_array.rs: Err(NeedsBacking));
 //   after   only those entries get their selection words back, read their LQDA image through the caller's function,
 //           and are refined again as full entries.
-static int scan_filter_squeezed(lc_scan* scan, Entry* const* es, const lc_predicate* pred) {
+// `d_target` is the selection refined in place (all_rows: it starts as every row and is written, not read), `d_counts`
+// the stride-2 survivor counts: the running selection and its counts for lc_scan_filter, a work buffer for
+// lc_scan_filter_or's terms.
+static int scan_filter_squeezed(lc_scan* scan, Entry* const* es, const lc_predicate* pred, uint32_t* d_target, bool all_rows,
+                                uint32_t* d_counts) {
   lc_ctx* ctx = scan->ctx;
   const uint64_t n = scan->n;
   struct Internal {  // the batch functions refuse squeezed entries unless squeeze code drives them
@@ -818,14 +828,14 @@ static int scan_filter_squeezed(lc_scan* scan, Entry* const* es, const lc_predic
   uint32_t* d_probe = scan->d_probe;
   uint32_t* d_save = scan->d_save;
   uint32_t* d_pcounts = scan->d_pcounts;
-  if (any_doubt && !scan->all_rows)
-    LC_CUDA_OK(cudaMemcpyAsync(d_save, scan->d_sel, scan->total_words * 4, cudaMemcpyDeviceToDevice, s));
+  if (any_doubt && !all_rows)
+    LC_CUDA_OK(cudaMemcpyAsync(d_save, d_target, scan->total_words * 4, cudaMemcpyDeviceToDevice, s));
   std::vector<uint32_t> pc(n * 2);
   for (int form = 1; form <= 2; ++form) {
     if (!n_doubt[form]) continue;
-    if (!scan->all_rows) LC_CUDA_OK(cudaMemcpyAsync(d_probe, scan->d_sel, scan->total_words * 4, cudaMemcpyDeviceToDevice, s));
+    if (!all_rows) LC_CUDA_OK(cudaMemcpyAsync(d_probe, d_target, scan->total_words * 4, cudaMemcpyDeviceToDevice, s));
     ctx->L()->scratch.reset();
-    LC_TRY(refine_batch(ctx, es, n, &probes[form], d_probe, scan->d_word_off, scan->all_rows, d_pcounts));
+    LC_TRY(refine_batch(ctx, es, n, &probes[form], d_probe, scan->d_word_off, all_rows, d_pcounts));
     LC_CUDA_OK(cudaMemcpyAsync(pc.data(), d_pcounts, n * 8, cudaMemcpyDeviceToHost, s));
     LC_CUDA_OK(cudaStreamSynchronize(s));
     ctx->d2h_bytes += n * 8;
@@ -834,19 +844,19 @@ static int scan_filter_squeezed(lc_scan* scan, Entry* const* es, const lc_predic
   }
   // ---- the predicate over the whole list ----
   ctx->L()->scratch.reset();
-  LC_TRY(refine_batch(ctx, es, n, pred, scan->d_sel, scan->d_word_off, scan->all_rows, scan->d_counts));
+  LC_TRY(refine_batch(ctx, es, n, pred, d_target, scan->d_word_off, all_rows, d_counts));
   // ---- entries the codes could not decide ----
   for (uint64_t i = 0; i < n; ++i) {
     if (es[i]->squeeze_kind && !backing[i]) ctx->squeeze_saved++;
     if (!backing[i]) continue;
     const uint64_t words = (static_cast<uint64_t>(scan->rows[i]) + 31) / 32;
-    if (!scan->all_rows)
-      LC_CUDA_OK(cudaMemcpyAsync(scan->d_sel + scan->word_off[i], d_save + scan->word_off[i], words * 4, cudaMemcpyDeviceToDevice, s));
+    if (!all_rows)
+      LC_CUDA_OK(cudaMemcpyAsync(d_target + scan->word_off[i], d_save + scan->word_off[i], words * 4, cudaMemcpyDeviceToDevice, s));
     Entry* full = nullptr;
     LC_TRY(squeeze_hydrate(ctx, es[i], &full));
     Entry* one[1] = {full};
     ctx->L()->scratch.reset();
-    const int rc = refine_batch(ctx, one, 1, pred, scan->d_sel, scan->d_word_off + i, scan->all_rows, scan->d_counts + 2 * i);
+    const int rc = refine_batch(ctx, one, 1, pred, d_target, scan->d_word_off + i, all_rows, d_counts + 2 * i);
     release_entry(ctx, full);
     LC_TRY(rc);
   }
@@ -864,8 +874,88 @@ int lc_scan_filter(lc_scan* scan, const lc_handle* handles, const lc_predicate* 
   bool any_squeezed = false;
   LC_TRY(scan_entries_cached(scan, handles, &es, &any_squeezed));
   if (any_squeezed) LC_TRY(refuse_in_list_on_squeezed(pred));
-  if (any_squeezed) LC_TRY(scan_filter_squeezed(scan, es, pred));
+  if (any_squeezed) LC_TRY(scan_filter_squeezed(scan, es, pred, scan->d_sel, scan->all_rows, scan->d_counts));
   else LC_TRY(refine_batch(ctx, es, scan->n, pred, scan->d_sel, scan->d_word_off, scan->all_rows, scan->d_counts));
+  scan->all_rows = false;
+  scan->counts_on_device = true;
+  scan->counts_cached = false;
+  return LC_OK;
+}
+
+// selection := selection & OR_d AND_{t in d} (valid_t & pred_t). Every term is refined exactly as lc_scan_filter would
+// refine it, but into the term buffer T, which starts each disjunct as the part of the selection no earlier disjunct has
+// accepted (S & ~A); k_sel_or then folds T into the accumulator A, or, after the last disjunct, writes S and its counts.
+// S is written by that last launch only, so a term refused anywhere in the list leaves the selection and counts as they were.
+int lc_scan_filter_or(lc_scan* scan, uint64_t n_terms, const lc_handle* const* handles, const lc_predicate* preds,
+                      const uint32_t* group) {
+  if (!scan || !handles || !preds || n_terms == 0) {
+    set_error("lc_scan_filter_or: NULL argument or no terms");
+    return LC_ERR_INVALID;
+  }
+  for (uint64_t t = 0; t < n_terms; ++t) {
+    if (!handles[t]) {
+      set_error("lc_scan_filter_or: term %llu has no handle list", (unsigned long long)t);
+      return LC_ERR_INVALID;
+    }
+    if (group && (t == 0 ? group[0] != 0u : (group[t] != group[t - 1] && group[t] != group[t - 1] + 1u))) {
+      set_error("lc_scan_filter_or: group must start at 0 and step by 0 or 1 (term %llu)", (unsigned long long)t);
+      return LC_ERR_INVALID;
+    }
+  }
+  lc_ctx* ctx = scan->ctx;
+  ScanGuard g(scan);
+  // every handle list is checked against the scan before anything runs
+  for (uint64_t t = 0; t < n_terms; ++t) {
+    Entry* const* es = nullptr;
+    LC_TRY(scan_entries_cached(scan, handles[t], &es));
+  }
+  cudaStream_t s = ctx->L()->stream;
+  const uint64_t n = scan->n;
+  const uint64_t sel_bytes = scan->total_words * 4 + 64;
+  if (!scan->d_rows) {  // set last, once everything else is in place (a failed first call leaves the rest for the next)
+    auto alloc = [](uint32_t** p, uint64_t bytes) { return *p || cudaMalloc(reinterpret_cast<void**>(p), bytes) == cudaSuccess; };
+    uint32_t* d_rows = nullptr;
+    if (!alloc(&scan->d_term, sel_bytes) || !alloc(&scan->d_acc, sel_bytes) || !alloc(&scan->d_tcounts, n * 8 + 16) ||
+        !alloc(&d_rows, n * 4 + 16)) {
+      cudaGetLastError();
+      set_error("lc_scan_filter_or: cudaMalloc for the work selections failed");
+      return LC_ERR_OOM;  // lc_scan_end frees whatever was allocated
+    }
+    // pageable source that lives as long as the scan
+    if (cudaMemcpyAsync(d_rows, scan->rows.data(), n * 4, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+      set_error("lc_scan_filter_or: upload of the row counts failed: %s", cudaGetErrorString(cudaGetLastError()));
+      cudaFree(d_rows);
+      return LC_ERR_CUDA;
+    }
+    scan->d_rows = d_rows;
+    ctx->h2d_bytes += n * 4;
+  }
+  const uint32_t n_groups = (group ? group[n_terms - 1] : static_cast<uint32_t>(n_terms - 1)) + 1u;
+  uint64_t t = 0;
+  for (uint32_t d = 0; d < n_groups; ++d) {
+    // T := S & ~A was left by the previous merge; the first disjunct starts from S itself
+    bool t_all = false;
+    if (d == 0) {
+      if (scan->all_rows) t_all = true;
+      else LC_CUDA_OK(cudaMemcpyAsync(scan->d_term, scan->d_sel, scan->total_words * 4, cudaMemcpyDeviceToDevice, s));
+    }
+    for (; t < n_terms && (group ? group[t] : t) == d; ++t) {
+      Entry* const* es = nullptr;
+      bool any_squeezed = false;
+      LC_TRY(scan_entries_cached(scan, handles[t], &es, &any_squeezed));
+      ctx->L()->scratch.reset();  // float terms decode into the lane scratch
+      if (any_squeezed) {
+        LC_TRY(refuse_in_list_on_squeezed(&preds[t]));
+        LC_TRY(scan_filter_squeezed(scan, es, &preds[t], scan->d_term, t_all, scan->d_tcounts));
+      } else {
+        LC_TRY(refine_batch(ctx, es, n, &preds[t], scan->d_term, scan->d_word_off, t_all, scan->d_tcounts));
+      }
+      t_all = false;
+    }
+    LC_CUDA_OK(launch_sel_or(scan->d_sel, scan->all_rows, scan->d_term, scan->d_acc, scan->d_word_off, scan->d_rows,
+                             static_cast<uint32_t>(n), d == 0, d + 1 == n_groups, scan->d_counts, s));
+    ctx->kernel_launches++;
+  }
   scan->all_rows = false;
   scan->counts_on_device = true;
   scan->counts_cached = false;
@@ -1113,6 +1203,10 @@ void lc_scan_end(lc_scan* scan) {
     if (scan->d_probe) cudaFree(scan->d_probe);
     if (scan->d_save) cudaFree(scan->d_save);
     if (scan->d_pcounts) cudaFree(scan->d_pcounts);
+    if (scan->d_term) cudaFree(scan->d_term);
+    if (scan->d_acc) cudaFree(scan->d_acc);
+    if (scan->d_tcounts) cudaFree(scan->d_tcounts);
+    if (scan->d_rows) cudaFree(scan->d_rows);
     if (scan->d_counts) cudaFree(scan->d_counts);
     if (scan->d_word_off) cudaFree(scan->d_word_off);
     fused_read_free(&scan->fused);

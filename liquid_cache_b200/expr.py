@@ -395,6 +395,58 @@ def _cast_chain_is_integer_identity(e, column_type: pa.DataType) -> bool:
     return True
 
 
+def _column_name(e) -> Optional[str]:
+    """The column under a cast chain (CastExpr / CastColumnExpr / TryCastExpr), None for anything else."""
+    while isinstance(e, CastExpr):
+        e = e.expr
+    return e.name if isinstance(e, Column) else None
+
+
+def _column_literal_leaf(e) -> Optional[str]:
+    """`extract_column_literal` (src/datafusion/src/reader/runtime/liquid_predicate.rs:45-68) for the leaves this library
+    lowers: a column (or a cast chain over one) compared with a literal, LIKE / NOT LIKE against a literal pattern, or an
+    IN list. Returns the column's name."""
+    if isinstance(e, BinaryExpr) and isinstance(e.right, Literal) and (e.op in _CMP_OPS or e.op in ("LikeMatch", "NotLikeMatch")):
+        return _column_name(e.left)
+    if isinstance(e, LikeExpr) and isinstance(e.pattern, Literal):
+        return _column_name(e.expr)
+    if isinstance(e, InListExpr):
+        return _column_name(e.expr)
+    return None
+
+
+def split_disjunction(expr) -> Optional[list]:
+    """An OR of column-literal leaves, or of AND groups of them, as `[[(column_name, leaf), ...], ...]` (one inner list per
+    disjunct, in the tree's left-to-right order) for `Scan.filter_or`; None for any other tree. The pure-OR case is
+    `extract_multi_column_or` (liquid_predicate.rs:12-43): the top node must be an OR, so there are at least two leaves.
+    AND is never distributed over OR: an AND group must hold leaves (or nested ANDs of leaves) only."""
+    if isinstance(expr, DynamicFilterPhysicalExpr):
+        expr = expr.current
+    if not (isinstance(expr, BinaryExpr) and expr.op == "OR"):
+        return None
+
+    def disjuncts(e, out) -> bool:
+        if isinstance(e, BinaryExpr) and e.op == "OR":
+            return disjuncts(e.left, out) and disjuncts(e.right, out)
+        group = []
+        if not conjuncts(e, group):
+            return False
+        out.append(group)
+        return True
+
+    def conjuncts(e, out) -> bool:
+        if isinstance(e, BinaryExpr) and e.op == "AND":
+            return conjuncts(e.left, out) and conjuncts(e.right, out)
+        name = _column_literal_leaf(e)
+        if name is None:
+            return False
+        out.append((name, e))
+        return True
+
+    out: list = []
+    return out if disjuncts(expr, out) else None
+
+
 def _supports_expr(expr, data_type, hint) -> bool:
     if isinstance(expr, BinaryExpr):
         return _supports_binary_expr(expr, data_type, hint)
