@@ -284,6 +284,30 @@ struct HostBuf {  // 64-byte aligned host allocation
 uint8_t* host_alloc(uint64_t bytes, bool force_pinned = false);  // force_pinned: a page-locked block even below 1 MiB
 void host_free(uint8_t* p);
 
+// A host_alloc block that goes back to host_free unless release() handed it to export_array (early returns, CUDA errors).
+struct HostBlock {
+  uint8_t* p = nullptr;
+  uint64_t bytes = 0;  // what the Arrow buffer holds; the allocation may be larger
+  HostBlock() = default;
+  HostBlock(uint64_t alloc_bytes, uint64_t b, bool force_pinned = false) : p(host_alloc(alloc_bytes, force_pinned)), bytes(b) {}
+  ~HostBlock() { host_free(p); }
+  HostBlock(HostBlock&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; }
+  HostBlock& operator=(HostBlock&& o) noexcept {
+    if (this != &o) {
+      host_free(p);
+      p = o.p;
+      bytes = o.bytes;
+      o.p = nullptr;
+    }
+    return *this;
+  }
+  HostBuf release() {  // ownership moves into an exported array
+    HostBuf r{p, bytes};
+    p = nullptr;
+    return r;
+  }
+};
+
 // Parsed view of an input array (borrowed pointers).
 struct ArrowIn {
   enum Kind { K_INT, K_BYTES, K_VIEW, K_DICT, K_FLOAT, K_DECIMAL } kind;
@@ -330,11 +354,6 @@ int register_codec(lc_ctx* ctx, uint64_t scope, const std::shared_ptr<FsstCodec>
 // str_host.cc
 int str_encode(lc_ctx* ctx, const ArrowIn& in, int32_t hint, uint64_t scope, Entry** out);
 int str_encode_many(lc_ctx* ctx, const std::vector<ArrowIn>& ins, int32_t hint, const uint64_t* scopes, std::vector<Entry*>* out);
-
-// Selection prepared for a launch.
-struct SelIn {
-  const uint8_t* bits = nullptr;  // host bits or nullptr
-};
 
 // scan_host.cc: batched operations over homogeneous entry lists (all int or all byte-view)
 struct PredOut {
@@ -390,7 +409,6 @@ struct FusedRead {
   uint8_t* a_buf = nullptr;      // scratch of the asynchronous form (scan_read_async)
   uint64_t a_cap = 0;
   ScanPlanHdr* h_hdr = nullptr;  // pinned
-  uint64_t fused_reads = 0, fallbacks = 0;
 };
 struct FusedDeviceOut {  // lc_scan_read_borrowed: the concatenated result left in the scan's own device buffer
   void* d_values = nullptr;

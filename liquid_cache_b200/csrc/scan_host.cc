@@ -1264,9 +1264,176 @@ int refine_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const lc_predic
   return LC_OK;
 }
 
+// ---- reads planned on the device -------------------------------------------------------------------
+// The survivors of a device-resident selection are sized, placed and decoded against capacities chosen before their counts
+// are known (k_scan_plan.cu, k_str_read_onepass); the 64-byte ScanPlanHdr (rows, bytes, overflow) says whether the
+// capacities sufficed. Used by the selective byte-view get (to_arrow_batch), scan_read_fused and scan_read_async.
+struct PlannedRead {
+  const uint32_t* sel_base;  // selection words
+  const uint64_t* sel_off;   // per entry: word offset into sel_base
+  const uint32_t* k2;        // per entry: surviving rows, at stride 2
+  uint64_t cap_rows, cap_bytes, cap_ulen;
+  bool onepass;              // byte views: the whole read is ONE kernel (k_str_read_onepass)
+  uint8_t* scratch;          // device, planned_layout(...).bytes
+  void* d_values;
+  int32_t* d_offsets;        // byte views: int32[cap_rows + 1]; integers: nullptr
+  ScanPlanHdr* d_hdr;
+};
+
+static uint64_t carve(uint64_t* o, uint64_t bytes) {
+  const uint64_t at = *o;
+  *o += round_up(bytes, 256);
+  return at;
+}
+
+// Offsets of the pieces of a read's device scratch; `bytes` is the total.
+struct PlannedLayout {
+  uint64_t status = 0, rowb = 0, vw = 0, ul = 0, bb = 0, cnt = 0, rowoff = 0, rowkey = 0, ulen = 0, bytes = 0;
+};
+static PlannedLayout planned_layout(uint64_t n, bool is_str, bool onepass, uint64_t cap_rows, uint64_t cap_ulen) {
+  PlannedLayout l;
+  if (onepass) {  // the status words of its chained scan are all the one-pass kernel needs
+    l.status = carve(&l.bytes, ((n + 7) / 8 + 2) * 8);
+    return l;
+  }
+  l.rowb = carve(&l.bytes, n * 8);
+  l.vw = carve(&l.bytes, n * 8);
+  l.ul = carve(&l.bytes, n * 8);
+  l.bb = carve(&l.bytes, n * 8);
+  l.cnt = carve(&l.bytes, n * 16);
+  if (is_str) {
+    l.rowoff = carve(&l.bytes, (cap_rows + n) * 4 + 16);
+    l.rowkey = carve(&l.bytes, cap_rows * 4 + 16);
+    l.ulen = carve(&l.bytes, cap_ulen * 4 + 16);
+  }
+  return l;
+}
+
+// Enqueues the read on the lane's stream without synchronising: the one-pass kernel, or the row plan followed by the
+// integer decode or by the four byte-view launches (sparse lengths, lengths, byte plan, decode).
+static int enqueue_planned_read(lc_ctx* ctx, const RefList* rl, uint64_t n, const PlannedRead& pr) {
+  cudaStream_t s = ctx->L()->stream;
+  const uint32_t nn = static_cast<uint32_t>(n);
+  const bool is_str = pr.d_offsets != nullptr;
+  const PlannedLayout l = planned_layout(n, is_str, pr.onepass, pr.cap_rows, pr.cap_ulen);
+  uint8_t* d = pr.scratch;
+  StrGatherIo g{};
+  g.io.refs = rl->d_refs;
+  g.io.sel_base = pr.sel_base;
+  g.io.sel_off = pr.sel_off;
+  g.k_hint = pr.k2;
+  g.out_offsets = pr.d_offsets;
+  g.out_bytes = static_cast<uint8_t*>(pr.d_values);
+  if (pr.onepass) {
+    LC_CUDA_OK(launch_str_read_onepass(nn, g, pr.cap_rows, pr.cap_bytes, pr.d_hdr, reinterpret_cast<unsigned long long*>(d + l.status), s));
+    ctx->kernel_launches++;
+    return LC_OK;
+  }
+  uint64_t* d_rowb = reinterpret_cast<uint64_t*>(d + l.rowb);
+  uint64_t* d_vw = reinterpret_cast<uint64_t*>(d + l.vw);
+  uint64_t* d_ul = reinterpret_cast<uint64_t*>(d + l.ul);
+  uint64_t* d_bb = reinterpret_cast<uint64_t*>(d + l.bb);
+  uint32_t* d_cnt = reinterpret_cast<uint32_t*>(d + l.cnt);
+  LC_CUDA_OK(cudaMemsetAsync(d_cnt, 0, n * 16, s));
+  LC_CUDA_OK(launch_scan_plan_rows(pr.k2, is_str ? rl->d_n_unique : nullptr, nn, pr.cap_rows, pr.cap_ulen, d_rowb, d_vw, d_ul, pr.d_hdr, s));
+  ctx->kernel_launches++;
+  g.io.out_off = d_rowb;
+  g.io.valid_off = d_vw;
+  g.io.counts = d_cnt;
+  g.io.counts_stride = 4;
+  if (!is_str) {
+    g.io.out_base = pr.d_values;
+    g.io.abort_flag = &pr.d_hdr->overflow;  // survivors beyond the capacity: the kernel returns without writing
+    LC_CUDA_OK(launch_int_scan(MODE_DECODE, nn, g.io, IntPredDesc{}, rl->max_blob, s));
+    ctx->kernel_launches++;
+    return LC_OK;
+  }
+  g.row_off_base = reinterpret_cast<uint32_t*>(d + l.rowoff);
+  g.row_key_base = reinterpret_cast<uint32_t*>(d + l.rowkey);
+  g.ulen_base = reinterpret_cast<uint32_t*>(d + l.ulen);
+  g.row_base = d_rowb;
+  g.ulen_off = d_ul;
+  g.byte_base = d_bb;
+  g.plan = pr.d_hdr;
+  g.sparse_max = 64;  // entries with up to 64 survivors: one warp each, no staging (k_str_lengths_sparse)
+  LC_CUDA_OK(launch_str_lengths_sparse(nn, g, s));
+  LC_CUDA_OK(launch_str_lengths(nn, g, rl->max_head, s));
+  LC_CUDA_OK(launch_scan_plan_bytes(d_cnt, nn, pr.cap_bytes, d_bb, g.out_offsets, pr.d_hdr, s));
+  LC_CUDA_OK(launch_str_decode(nn, g, s));
+  ctx->kernel_launches += 4;
+  return LC_OK;
+}
+
+// The host's half of a planned read: the header, the offsets (byte views) and a speculative prefix of the values come down
+// with ONE synchronisation; a result larger than that prefix is fetched whole in a second round trip (rare). `value_width`
+// is the integers' bytes per value (byte views: 0, their size is in the header). When the header reports an overflow
+// nothing more is fetched or counted: the caller decides.
+struct PlannedHost {
+  ScanPlanHdr hdr{};
+  HostBlock offsets, values;
+};
+static int download_planned(lc_ctx* ctx, ScanPlanHdr* h_hdr, const PlannedRead& pr, uint32_t value_width, uint64_t spec_rows,
+                            uint64_t spec_bytes, PlannedHost* out) {
+  cudaStream_t s = ctx->L()->stream;
+  const bool is_str = pr.d_offsets != nullptr;
+  const uint64_t pre_rows = std::min(spec_rows, pr.cap_rows), pre_bytes = std::min(spec_bytes, pr.cap_bytes);
+  if (is_str) out->offsets = HostBlock((spec_rows + 1) * 4 + 64, 0, true);
+  out->values = HostBlock(spec_bytes + 64, 0, true);
+  if ((is_str && !out->offsets.p) || !out->values.p) {
+    set_error("host allocation failed");
+    return LC_ERR_OOM;
+  }
+  LC_CUDA_OK(cudaMemcpyAsync(h_hdr, pr.d_hdr, sizeof(ScanPlanHdr), cudaMemcpyDeviceToHost, s));
+  if (is_str) LC_CUDA_OK(cudaMemcpyAsync(out->offsets.p, pr.d_offsets, (pre_rows + 1) * 4, cudaMemcpyDeviceToHost, s));
+  if (pre_bytes) LC_CUDA_OK(cudaMemcpyAsync(out->values.p, pr.d_values, pre_bytes, cudaMemcpyDeviceToHost, s));
+  LC_CUDA_OK(cudaStreamSynchronize(s));
+  out->hdr = *h_hdr;
+  if (out->hdr.overflow) return LC_OK;
+  const uint64_t rows = out->hdr.rows, bytes = is_str ? out->hdr.bytes : rows * value_width;
+  ctx->d2h_bytes += sizeof(ScanPlanHdr) + (is_str ? (pre_rows + 1) * 4 : 0) + pre_bytes;
+  if (rows > spec_rows || bytes > spec_bytes) {
+    // offsets that covered the whole row capacity are complete (the selective get knows its rows); the rest comes again
+    const bool offsets_again = is_str && spec_rows < pr.cap_rows;
+    if (offsets_again) out->offsets = HostBlock((rows + 1) * 4 + 64, 0, true);
+    out->values = HostBlock(bytes + 64, 0, true);
+    if ((offsets_again && !out->offsets.p) || !out->values.p) {
+      set_error("host allocation failed");
+      return LC_ERR_OOM;
+    }
+    if (offsets_again) LC_CUDA_OK(cudaMemcpyAsync(out->offsets.p, pr.d_offsets, (rows + 1) * 4, cudaMemcpyDeviceToHost, s));
+    LC_CUDA_OK(cudaMemcpyAsync(out->values.p, pr.d_values, bytes, cudaMemcpyDeviceToHost, s));
+    LC_CUDA_OK(cudaStreamSynchronize(s));
+    ctx->d2h_bytes += (offsets_again ? (rows + 1) * 4 : 0) + bytes;
+  }
+  if (is_str) {
+    reinterpret_cast<int32_t*>(out->offsets.p)[rows] = static_cast<int32_t>(bytes);
+    out->offsets.bytes = (rows + 1) * 4;
+  }
+  out->values.bytes = bytes;
+  return LC_OK;
+}
+
+// Makes a scan's device buffer hold `need` bytes; a new allocation gets `headroom` more. LC_INTERNAL_FALLBACK when
+// cudaMalloc fails.
+static int grow_device(cudaStream_t s, uint8_t** buf, uint64_t* cap, uint64_t need, uint64_t headroom) {
+  if (need <= *cap) return LC_OK;
+  if (*buf) {
+    LC_CUDA_OK(cudaStreamSynchronize(s));
+    cudaFree(*buf);
+    *buf = nullptr;
+    *cap = 0;
+  }
+  if (cudaMalloc(reinterpret_cast<void**>(buf), need + headroom) != cudaSuccess) {
+    cudaGetLastError();
+    return LC_INTERNAL_FALLBACK;
+  }
+  *cap = need + headroom;
+  return LC_OK;
+}
+
 // ---- get / filter ----------------------------------------------------------------------------------
-static int finish_bytes_array(const Entry* proto, uint64_t rows, uint64_t nulls, HostBuf validity, HostBuf offsets,
-                              HostBuf views, HostBuf data, ArrowSchema* out_schema, ArrowArray* out_array);
+static int finish_bytes_array(const Entry* proto, uint64_t rows, uint64_t nulls, HostBlock validity, HostBlock offsets,
+                              HostBlock views, HostBlock data, ArrowSchema* out_schema, ArrowArray* out_array);
 
 int to_arrow_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const uint8_t* const* sel_bits,
                    const DevSel* dev_sel, ArrowSchema* out_schema, ArrowArray* out_array, const DeviceOut* dev_out) {
@@ -1341,9 +1508,8 @@ int to_arrow_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const uint8_t
   // granularity ON THE DEVICE (k_concat_validity; entries without nulls read as all ones) and the finished bitmap is
   // copied to the host — no host loop over rows or entries.
   const uint64_t cat_bytes = round_up(((rows + 31) / 32) * 4 + 16, 256);
-  auto concat_validity_device = [&](const ScanIo& io, uint8_t* d_up, uint8_t* d_cat, HostBuf* validity) -> int {
-    validity->bytes = (rows + 7) / 8;
-    validity->p = host_alloc(round_up(validity->bytes, 4));
+  auto concat_validity_device = [&](const ScanIo& io, uint8_t* d_up, uint8_t* d_cat, HostBlock* validity) -> int {
+    *validity = HostBlock(round_up((rows + 7) / 8, 4), (rows + 7) / 8);
     if (!validity->p) {
       set_error("host allocation failed");
       return LC_ERR_OOM;
@@ -1438,49 +1604,31 @@ int to_arrow_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const uint8_t
       ctx->kernel_launches++;
       d_result = d_wide;
     }
-    HostBuf values{host_alloc(rows * out_tb), rows * out_tb};
+    HostBlock values(rows * out_tb, rows * out_tb);
     if (!values.p) {
       set_error("host allocation of %llu bytes failed", (unsigned long long)(rows * out_tb));
       return LC_ERR_OOM;
     }
-    {
-      cudaError_t ce = cudaMemcpyAsync(h_dn, d_dn, dn_counts, cudaMemcpyDeviceToHost, s);
-      if (ce == cudaSuccess && rows) ce = cudaMemcpyAsync(values.p, d_result, rows * out_tb, cudaMemcpyDeviceToHost, s);
-      if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-      if (ce != cudaSuccess) {
-        host_free(values.p);  // the result buffer goes back on the error path too
-        set_error("CUDA error in integer get: %s", cudaGetErrorString(ce));
-        return LC_ERR_CUDA;
-      }
-    }
+    LC_CUDA_OK(cudaMemcpyAsync(h_dn, d_dn, dn_counts, cudaMemcpyDeviceToHost, s));
+    if (rows) LC_CUDA_OK(cudaMemcpyAsync(values.p, d_result, rows * out_tb, cudaMemcpyDeviceToHost, s));
+    LC_CUDA_OK(cudaStreamSynchronize(s));
     ctx->d2h_bytes += dn_counts + rows * out_tb;
     const uint32_t* h_counts = reinterpret_cast<const uint32_t*>(h_dn);
     uint64_t nulls = 0;
     for (uint64_t i = 0; i < n; ++i) {
       if (h_counts[4 * i] != sp.k[i]) {
-        host_free(values.p);
         set_error("internal: selected-row count mismatch on entry %llu", (unsigned long long)i);
         return LC_ERR_INVALID;
       }
       nulls += h_counts[4 * i + 1];
     }
-    HostBuf validity;
+    HostBlock validity;
     if (nulls) {  // second, small round trip only when the result has nulls
-      int rc = concat_validity_device(io, d_up, d_cat, &validity);
-      if (rc == LC_OK && cudaStreamSynchronize(s) != cudaSuccess) {
-        set_error("CUDA error while joining validity: %s", cudaGetErrorString(cudaGetLastError()));
-        rc = LC_ERR_CUDA;
-      }
-      if (rc != LC_OK) {
-        host_free(values.p);
-        host_free(validity.p);
-        return rc;
-      }
+      LC_TRY(concat_validity_device(io, d_up, d_cat, &validity));
+      LC_CUDA_OK(cudaStreamSynchronize(s));
     }
     export_schema(proto->arrow_format, "", out_schema);
-    std::vector<HostBuf> bufs;
-    bufs.push_back(validity);
-    bufs.push_back(values);
+    std::vector<HostBuf> bufs{validity.release(), values.release()};
     export_array(static_cast<int64_t>(rows), static_cast<int64_t>(nulls), std::move(bufs), nullptr, out_array);
     return LC_OK;
   }
@@ -1502,17 +1650,17 @@ int to_arrow_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const uint8_t
       const uint64_t cap_bytes = bound;
       const uint64_t up_tab = round_up(n * 16, 256);  // word_off[n] (u64) | k[n] at stride 2 (u32 pairs)
       const uint64_t up_sel1 = round_up(sp.sel_words * 4, 256);
-      const uint64_t dv_status = round_up(((n + 7) / 8 + 2) * 8, 256);
+      const uint64_t dv_plan = planned_layout(n, true, true, rows, 0).bytes;
       const uint64_t dv_off = round_up((rows + 1) * 4, 256), dv_val = round_up(cap_bytes + 16, 256);
-      LC_TRY(sc.reserve(up_tab + up_sel1 + dv_status + 256 + dv_off + dv_val + 1024, up_tab + 256 + 1024));
+      LC_TRY(sc.reserve(up_tab + up_sel1 + dv_plan + 256 + dv_off + dv_val + 1024, up_tab + 256 + 1024));
       uint8_t* h_up = sc.host(up_tab);
       ScanPlanHdr* h_hdr = reinterpret_cast<ScanPlanHdr*>(sc.host(256));
       uint8_t* d_up = sc.dev(up_tab + up_sel1);
-      uint8_t* d_status = sc.dev(dv_status);
+      uint8_t* d_plan = sc.dev(dv_plan);
       ScanPlanHdr* d_hdr = reinterpret_cast<ScanPlanHdr*>(sc.dev(256));
-      uint8_t* d_off = sc.dev(dv_off);
+      int32_t* d_off = reinterpret_cast<int32_t*>(sc.dev(dv_off));
       uint8_t* d_val = sc.dev(dv_val);
-      if (!h_up || !h_hdr || !d_up || !d_status || !d_hdr || !d_off || !d_val) {
+      if (!h_up || !h_hdr || !d_up || !d_plan || !d_hdr || !d_off || !d_val) {
         set_error("to_arrow: scratch exhausted");
         return LC_ERR_OOM;
       }
@@ -1526,67 +1674,31 @@ int to_arrow_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const uint8_t
       LC_CUDA_OK(cudaMemcpyAsync(d_up, h_up, n * 16, cudaMemcpyHostToDevice, s));
       ctx->h2d_bytes += n * 16;
       LC_TRY(upload_selection(ctx, sp, d_up + up_tab, s));
-      StrGatherIo g{};
-      g.io.refs = rl->d_refs;
-      g.io.sel_base = reinterpret_cast<const uint32_t*>(d_up + up_tab);
-      g.io.sel_off = reinterpret_cast<const uint64_t*>(d_up);
-      g.k_hint = reinterpret_cast<const uint32_t*>(d_up + n * 8);
-      g.out_offsets = reinterpret_cast<int32_t*>(d_off);
-      g.out_bytes = d_val;
-      LC_CUDA_OK(launch_str_read_onepass(static_cast<uint32_t>(n), g, rows, cap_bytes, d_hdr, reinterpret_cast<unsigned long long*>(d_status), s));
-      ctx->kernel_launches++;
+      PlannedRead pr{};
+      pr.sel_base = reinterpret_cast<const uint32_t*>(d_up + up_tab);
+      pr.sel_off = reinterpret_cast<const uint64_t*>(d_up);
+      pr.k2 = reinterpret_cast<const uint32_t*>(d_up + n * 8);
+      pr.cap_rows = rows;
+      pr.cap_bytes = cap_bytes;
+      pr.onepass = true;
+      pr.scratch = d_plan;
+      pr.d_values = d_val;
+      pr.d_offsets = d_off;
+      pr.d_hdr = d_hdr;
+      LC_TRY(enqueue_planned_read(ctx, rl, n, pr));
       double& ratio = ctx->L()->onepass_bytes_per_row;
       const uint64_t spec = std::min<uint64_t>(cap_bytes, static_cast<uint64_t>(static_cast<double>(rows) * ratio * 1.25) + 4096);
-      HostBuf offsets{host_alloc((rows + 1) * 4 + 64, true), (rows + 1) * 4};
-      HostBuf data{host_alloc(spec + 64, true), spec};
-      auto drop = [&]() {
-        host_free(offsets.p);
-        host_free(data.p);
-      };
-      if (!offsets.p || !data.p) {
-        drop();
-        set_error("host allocation failed");
-        return LC_ERR_OOM;
-      }
-      cudaError_t ce = cudaMemcpyAsync(h_hdr, d_hdr, sizeof(ScanPlanHdr), cudaMemcpyDeviceToHost, s);
-      if (ce == cudaSuccess) ce = cudaMemcpyAsync(offsets.p, d_off, (rows + 1) * 4, cudaMemcpyDeviceToHost, s);
-      if (ce == cudaSuccess && spec) ce = cudaMemcpyAsync(data.p, d_val, spec, cudaMemcpyDeviceToHost, s);
-      if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-      tr.mark("one-pass read + the one synchronisation");
-      if (ce != cudaSuccess) {
-        drop();
-        set_error("CUDA error in the one-pass read: %s", cudaGetErrorString(ce));
-        return LC_ERR_CUDA;
-      }
-      const ScanPlanHdr hdr = *h_hdr;
-      if (hdr.overflow || hdr.rows != rows) {  // cannot happen with an upper bound as the capacity: refuse rather than guess
-        drop();
-        set_error("internal: one-pass read reported rows %llu (expected %llu), overflow %u", (unsigned long long)hdr.rows,
-                  (unsigned long long)rows, hdr.overflow);
+      PlannedHost res;
+      LC_TRY(download_planned(ctx, h_hdr, pr, 0, rows, spec, &res));
+      tr.mark("one-pass read + its download");
+      if (res.hdr.overflow || res.hdr.rows != rows) {  // cannot happen with an upper bound as the capacity: refuse rather than guess
+        set_error("internal: one-pass read reported rows %llu (expected %llu), overflow %u", (unsigned long long)res.hdr.rows,
+                  (unsigned long long)rows, res.hdr.overflow);
         return LC_ERR_INVALID;
       }
-      const uint64_t bytes = hdr.bytes;
-      ctx->d2h_bytes += sizeof(ScanPlanHdr) + (rows + 1) * 4 + spec;
-      if (bytes > spec) {  // larger than the speculative download: fetch the values whole (a second round trip, rare)
-        host_free(data.p);
-        data = HostBuf{host_alloc(bytes + 64, true), bytes};
-        if (!data.p) {
-          drop();
-          set_error("host allocation failed");
-          return LC_ERR_OOM;
-        }
-        ce = cudaMemcpyAsync(data.p, d_val, bytes, cudaMemcpyDeviceToHost, s);
-        if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-        if (ce != cudaSuccess) {
-          drop();
-          set_error("CUDA error in the one-pass read: %s", cudaGetErrorString(ce));
-          return LC_ERR_CUDA;
-        }
-        ctx->d2h_bytes += bytes;
-      }
-      data.bytes = bytes;
-      ratio = std::max(8.0, static_cast<double>(bytes) / static_cast<double>(rows));
-      return finish_bytes_array(proto, rows, 0, HostBuf{}, offsets, HostBuf{}, data, out_schema, out_array);
+      ratio = std::max(8.0, static_cast<double>(res.values.bytes) / static_cast<double>(rows));
+      return finish_bytes_array(proto, rows, 0, HostBlock{}, std::move(res.offsets), HostBlock{}, std::move(res.values), out_schema,
+                                out_array);
     }
   }
 
@@ -1719,19 +1831,12 @@ int to_arrow_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const uint8_t
   g.out_bytes = d_res + round_up(off_bytes, 256);
   uint8_t* d_views = g.out_bytes + round_up(total_bytes + 16, 256);
   // view types ship 16-byte views built on the device instead of the offsets
-  HostBuf offsets{want_views ? nullptr : host_alloc(off_bytes), want_views ? 0 : off_bytes};
-  HostBuf views{want_views ? host_alloc(view_bytes + 16) : nullptr, view_bytes};
-  HostBuf data{host_alloc(total_bytes ? total_bytes : 1), total_bytes};
-  HostBuf validity;
-  auto drop_host = [&]() {
-    host_free(offsets.p);
-    host_free(views.p);
-    host_free(data.p);
-    host_free(validity.p);
-  };
+  HostBlock offsets = want_views ? HostBlock() : HostBlock(off_bytes, off_bytes);
+  HostBlock views = want_views ? HostBlock(view_bytes + 16, view_bytes) : HostBlock();
+  HostBlock data(total_bytes ? total_bytes : 1, total_bytes);
+  HostBlock validity;
   if ((!want_views && !offsets.p) || (want_views && !views.p) || !data.p) {
     cudaFreeAsync(d_res, s);
-    drop_host();
     set_error("host allocation failed");
     return LC_ERR_OOM;
   }
@@ -1761,20 +1866,18 @@ int to_arrow_batch(lc_ctx* ctx, Entry* const* entries, uint64_t n, const uint8_t
     ce = cudaMemcpyAsync(data.p, g.out_bytes, total_bytes, cudaMemcpyDeviceToHost, s);
   cudaFreeAsync(d_res, s);
   if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-  if (ce != cudaSuccess || rc != LC_OK) {
-    drop_host();
-    if (ce != cudaSuccess) {
-      set_error("CUDA error in byte-view decode: %s", cudaGetErrorString(ce));
-      return LC_ERR_CUDA;
-    }
-    return rc;
+  if (ce != cudaSuccess) {
+    set_error("CUDA error in byte-view decode: %s", cudaGetErrorString(ce));
+    return LC_ERR_CUDA;
   }
+  LC_TRY(rc);
   tr.mark("decode kernel + result D2H");
   ctx->kernel_launches++;
   ctx->h2d_bytes += n * 8;
   ctx->d2h_bytes += (want_views ? view_bytes : rows * 4) + (fixed_w ? 0 : total_bytes);
   if (!want_views) reinterpret_cast<int32_t*>(offsets.p)[rows] = static_cast<int32_t>(total_bytes);
-  return finish_bytes_array(proto, rows, nulls, validity, offsets, views, data, out_schema, out_array);
+  return finish_bytes_array(proto, rows, nulls, std::move(validity), std::move(offsets), std::move(views), std::move(data), out_schema,
+                            out_array);
 }
 
 // ---- get over a device-resident selection with ONE host synchronisation ----------------------------------------
@@ -1805,186 +1908,63 @@ int scan_read_fused(lc_ctx* ctx, FusedRead* fr, Entry* const* entries, uint64_t 
   cudaStream_t s = ctx->L()->stream;
   Tracer tr("scan_read_fused");
 
-  const uint64_t cap_rows = fr->spec_rows + fr->spec_rows / 2 + 4096;
-  const uint64_t cap_bytes = is_int ? 0 : fr->spec_bytes + fr->spec_bytes / 2 + (64u << 10);
-  const uint64_t cap_ulen = is_int ? 0 : fr->spec_ulen + fr->spec_ulen / 2 + (64u << 10);
-  // one device allocation, carved: header | 4 offset arrays | counts4 | scratch | result
-  uint64_t o = 0;
-  auto take = [&](uint64_t bytes) { const uint64_t at = o; o += round_up(bytes, 256); return at; };
+  PlannedRead pr{};
+  pr.sel_base = d_sel;
+  pr.sel_off = d_word_off;
+  pr.k2 = d_counts2;
+  pr.cap_rows = fr->spec_rows + fr->spec_rows / 2 + 4096;
+  pr.cap_bytes = is_int ? pr.cap_rows * tb : fr->spec_bytes + fr->spec_bytes / 2 + (64u << 10);
+  pr.cap_ulen = is_int ? 0 : fr->spec_ulen + fr->spec_ulen / 2 + (64u << 10);
   // the previous read of this scan left a handful of survivors per entry: one kernel does the whole read (k_str_read_onepass)
-  const bool onepass = is_str && fr->spec_rows <= 8ull * n;
-  const uint64_t o_hdr = take(256), o_rowb = take(n * 8), o_vw = take(n * 8), o_ul = take(n * 8), o_bb = take(n * 8);
-  const uint64_t o_cnt = take(n * 16);
-  const uint64_t o_status = onepass ? take(((n + 7) / 8 + 2) * 8) : 0;
-  const uint64_t o_rowoff = (is_str && !onepass) ? take((cap_rows + n) * 4 + 16) : 0, o_rowkey = (is_str && !onepass) ? take(cap_rows * 4 + 16) : 0;
-  const uint64_t o_ulen = (is_str && !onepass) ? take(cap_ulen * 4 + 16) : 0;
-  const uint64_t o_off = is_str ? take((cap_rows + 1) * 4) : 0;
-  const uint64_t o_val = take(is_int ? cap_rows * tb + 16 : cap_bytes + 16);
-  if (o > fr->d_cap) {
-    if (fr->d_buf) {
-      LC_CUDA_OK(cudaStreamSynchronize(s));
-      cudaFree(fr->d_buf);
-      fr->d_buf = nullptr;
-      fr->d_cap = 0;
-    }
-    const uint64_t want = o + o / 4;
-    if (cudaMalloc(reinterpret_cast<void**>(&fr->d_buf), want) != cudaSuccess) {
-      cudaGetLastError();
-      return LC_INTERNAL_FALLBACK;
-    }
-    fr->d_cap = want;
-  }
+  pr.onepass = is_str && fr->spec_rows <= 8ull * n;
+  // one device allocation, carved: the read's scratch | header | offsets | values (a borrowed result stays here)
+  uint64_t o = planned_layout(n, is_str, pr.onepass, pr.cap_rows, pr.cap_ulen).bytes;
+  const uint64_t o_hdr = carve(&o, 256);
+  const uint64_t o_off = is_str ? carve(&o, (pr.cap_rows + 1) * 4) : 0;
+  const uint64_t o_val = carve(&o, pr.cap_bytes + 16);
+  LC_TRY(grow_device(s, &fr->d_buf, &fr->d_cap, o, o / 4));
   if (!fr->h_hdr && cudaHostAlloc(reinterpret_cast<void**>(&fr->h_hdr), 256, cudaHostAllocDefault) != cudaSuccess) {
     cudaGetLastError();
     return LC_INTERNAL_FALLBACK;
   }
   uint8_t* d = fr->d_buf;
-  ScanPlanHdr* d_hdr = reinterpret_cast<ScanPlanHdr*>(d + o_hdr);
-  uint64_t* d_rowb = reinterpret_cast<uint64_t*>(d + o_rowb);
-  uint64_t* d_vw = reinterpret_cast<uint64_t*>(d + o_vw);
-  uint64_t* d_ul = reinterpret_cast<uint64_t*>(d + o_ul);
-  uint64_t* d_bb = reinterpret_cast<uint64_t*>(d + o_bb);
-  uint32_t* d_cnt = reinterpret_cast<uint32_t*>(d + o_cnt);
-  if (!onepass) {
-    LC_CUDA_OK(cudaMemsetAsync(d_cnt, 0, n * 16, s));
-    LC_CUDA_OK(launch_scan_plan_rows(d_counts2, is_str ? rl->d_n_unique : nullptr, static_cast<uint32_t>(n), cap_rows, cap_ulen, d_rowb,
-                                     d_vw, d_ul, d_hdr, s));
-    ctx->kernel_launches++;
-  }
-  ScanIo io{};
-  io.refs = rl->d_refs;
-  io.sel_base = d_sel;
-  io.sel_off = d_word_off;
-  io.out_off = d_rowb;
-  io.valid_base = nullptr;
-  io.valid_off = d_vw;
-  io.counts = d_cnt;
-  io.counts_stride = 4;
-  HostBuf values, offsets;
-  const uint64_t spec_rows = fr->spec_rows + fr->spec_rows / 8 + 64;
-  const uint64_t spec_bytes = fr->spec_bytes + fr->spec_bytes / 8 + 4096;
-  if (is_int) {
-    io.out_base = d + o_val;
-    IntPredDesc ip{};
-    io.abort_flag = &d_hdr->overflow;  // survivors beyond the capacity: the kernel returns without writing
-    LC_CUDA_OK(launch_int_scan(MODE_DECODE, static_cast<uint32_t>(n), io, ip, rl->max_blob, s));
-    ctx->kernel_launches++;
-    LC_CUDA_OK(cudaMemcpyAsync(fr->h_hdr, d_hdr, sizeof(ScanPlanHdr), cudaMemcpyDeviceToHost, s));
-    if (!dev_out) {
-      values = HostBuf{host_alloc(spec_rows * tb + 64, true), spec_rows * tb};
-      if (!values.p) return LC_ERR_OOM;
-      LC_CUDA_OK(cudaMemcpyAsync(values.p, d + o_val, std::min(spec_rows, cap_rows) * tb, cudaMemcpyDeviceToHost, s));
-    }
-  } else {
-    StrGatherIo g{};
-    g.io = io;
-    g.row_off_base = reinterpret_cast<uint32_t*>(d + o_rowoff);
-    g.row_key_base = reinterpret_cast<uint32_t*>(d + o_rowkey);
-    g.ulen_base = reinterpret_cast<uint32_t*>(d + o_ulen);
-    g.row_base = d_rowb;
-    g.ulen_off = d_ul;
-    g.byte_base = d_bb;
-    g.k_hint = d_counts2;
-    g.plan = d_hdr;
-    g.sparse_max = 64;  // entries with up to 64 survivors: one warp each, no staging (k_str_lengths_sparse)
-    g.out_offsets = reinterpret_cast<int32_t*>(d + o_off);
-    g.out_bytes = d + o_val;
-    if (onepass) {
-      LC_CUDA_OK(launch_str_read_onepass(static_cast<uint32_t>(n), g, cap_rows, cap_bytes, d_hdr,
-                                         reinterpret_cast<unsigned long long*>(d + o_status), s));
-      ctx->kernel_launches++;
-    } else {
-      LC_CUDA_OK(launch_str_lengths_sparse(static_cast<uint32_t>(n), g, s));
-      LC_CUDA_OK(launch_str_lengths(static_cast<uint32_t>(n), g, rl->max_head, s));
-      LC_CUDA_OK(launch_scan_plan_bytes(d_cnt, static_cast<uint32_t>(n), cap_bytes, d_bb, g.out_offsets, d_hdr, s));
-      LC_CUDA_OK(launch_str_decode(static_cast<uint32_t>(n), g, s));
-      ctx->kernel_launches += 4;
-    }
-    LC_CUDA_OK(cudaMemcpyAsync(fr->h_hdr, d_hdr, sizeof(ScanPlanHdr), cudaMemcpyDeviceToHost, s));
-    if (!dev_out) {
-      offsets = HostBuf{host_alloc((spec_rows + 1) * 4 + 64, true), (spec_rows + 1) * 4};
-      values = HostBuf{host_alloc(spec_bytes + 64, true), spec_bytes};
-      if (!offsets.p || !values.p) {
-        host_free(offsets.p);
-        host_free(values.p);
-        return LC_ERR_OOM;
-      }
-      LC_CUDA_OK(cudaMemcpyAsync(offsets.p, g.out_offsets, (std::min(spec_rows, cap_rows) + 1) * 4, cudaMemcpyDeviceToHost, s));
-      LC_CUDA_OK(cudaMemcpyAsync(values.p, g.out_bytes, std::min(spec_bytes, cap_bytes), cudaMemcpyDeviceToHost, s));
-    }
-  }
+  pr.scratch = d;
+  pr.d_values = d + o_val;
+  pr.d_offsets = is_str ? reinterpret_cast<int32_t*>(d + o_off) : nullptr;
+  pr.d_hdr = reinterpret_cast<ScanPlanHdr*>(d + o_hdr);
+  LC_TRY(enqueue_planned_read(ctx, rl, n, pr));
   tr.mark("launches");
-  cudaError_t ce = cudaStreamSynchronize(s);
-  tr.mark("the one synchronisation");
-  const ScanPlanHdr hdr = *fr->h_hdr;
-  auto drop = [&]() {
-    host_free(offsets.p);
-    host_free(values.p);
-  };
-  if (ce != cudaSuccess) {
-    drop();
-    set_error("CUDA error in the device-planned read: %s", cudaGetErrorString(ce));
-    return LC_ERR_CUDA;
+  PlannedHost res;
+  if (dev_out) {  // the result stays in the scan's device buffer (valid until the next read of this scan)
+    LC_CUDA_OK(cudaMemcpyAsync(fr->h_hdr, pr.d_hdr, sizeof(ScanPlanHdr), cudaMemcpyDeviceToHost, s));
+    LC_CUDA_OK(cudaStreamSynchronize(s));
+    res.hdr = *fr->h_hdr;
+    if (!res.hdr.overflow) ctx->d2h_bytes += sizeof(ScanPlanHdr);
+  } else {
+    const uint64_t spec_rows = fr->spec_rows + fr->spec_rows / 8 + 64;
+    const uint64_t spec_bytes = is_int ? spec_rows * tb : fr->spec_bytes + fr->spec_bytes / 8 + 4096;
+    LC_TRY(download_planned(ctx, fr->h_hdr, pr, tb, spec_rows, spec_bytes, &res));
   }
-  if (hdr.overflow) {  // a capacity was short: the kernels did nothing; let the host-planned path answer and re-teach the sizes
-    drop();
+  tr.mark("download");
+  if (res.hdr.overflow) {  // a capacity was short: the kernels did nothing; let the host-planned path answer and re-teach the sizes
     fr->have_spec = false;
-    fr->fallbacks++;
     return LC_INTERNAL_FALLBACK;
   }
-  const uint64_t rows = hdr.rows, bytes = is_int ? rows * tb : hdr.bytes;
-  if (dev_out) {  // the result stays in the scan's device buffer (valid until the next read of this scan)
-    ctx->d2h_bytes += sizeof(ScanPlanHdr);
-    fr->spec_rows = rows;
-    fr->spec_bytes = is_int ? 0 : bytes;
-    if (!onepass) fr->spec_ulen = hdr.ulen_words;
-    fr->fused_reads++;
-    dev_out->d_values = d + o_val;
-    dev_out->d_offsets = is_int ? nullptr : d + o_off;
+  const uint64_t rows = res.hdr.rows, bytes = is_int ? rows * tb : res.hdr.bytes;
+  fr->spec_rows = rows;
+  fr->spec_bytes = is_int ? 0 : bytes;
+  if (!pr.onepass) fr->spec_ulen = res.hdr.ulen_words;  // the one-pass kernel uses no dictionary-length scratch: keep what the general path learnt
+  if (dev_out) {
+    dev_out->d_values = pr.d_values;
+    dev_out->d_offsets = pr.d_offsets;
     dev_out->rows = rows;
     dev_out->value_bytes = bytes;
     return LC_OK;
   }
-  ctx->d2h_bytes += sizeof(ScanPlanHdr) + (is_int ? std::min(spec_rows, cap_rows) * tb
-                                                  : (std::min(spec_rows, cap_rows) + 1) * 4 + std::min(spec_bytes, cap_bytes));
-  if (rows > spec_rows || (!is_int && bytes > spec_bytes)) {
-    // this read is larger than the speculative download: fetch it whole (a second round trip, rare)
-    drop();
-    if (is_int) {
-      values = HostBuf{host_alloc(rows * tb + 64, true), rows * tb};
-      if (!values.p) return LC_ERR_OOM;
-      LC_CUDA_OK(cudaMemcpyAsync(values.p, d + o_val, rows * tb, cudaMemcpyDeviceToHost, s));
-    } else {
-      offsets = HostBuf{host_alloc((rows + 1) * 4 + 64, true), (rows + 1) * 4};
-      values = HostBuf{host_alloc(bytes + 64, true), bytes};
-      if (!offsets.p || !values.p) {
-        drop();
-        return LC_ERR_OOM;
-      }
-      LC_CUDA_OK(cudaMemcpyAsync(offsets.p, d + o_off, (rows + 1) * 4, cudaMemcpyDeviceToHost, s));
-      LC_CUDA_OK(cudaMemcpyAsync(values.p, d + o_val, bytes, cudaMemcpyDeviceToHost, s));
-    }
-    LC_CUDA_OK(cudaStreamSynchronize(s));
-    ctx->d2h_bytes += (is_int ? 0 : (rows + 1) * 4) + bytes;
-    tr.mark("second download");
-  }
-  fr->spec_rows = rows;
-  fr->spec_bytes = is_int ? 0 : bytes;
-  if (!onepass) fr->spec_ulen = hdr.ulen_words;  // the one-pass kernel uses no dictionary-length scratch: keep what the general path learnt
-  fr->fused_reads++;
   export_schema(proto->arrow_format, "", out_schema);
-  std::vector<HostBuf> bufs;
-  bufs.push_back(HostBuf{});  // no validity: the list has no nulls
-  if (is_int) {
-    values.bytes = rows * tb;
-    bufs.push_back(values);
-  } else {
-    reinterpret_cast<int32_t*>(offsets.p)[rows] = static_cast<int32_t>(bytes);
-    offsets.bytes = (rows + 1) * 4;
-    values.bytes = bytes;
-    bufs.push_back(offsets);
-    bufs.push_back(values);
-  }
+  std::vector<HostBuf> bufs(1);  // no validity: the list has no nulls
+  if (is_str) bufs.push_back(res.offsets.release());
+  bufs.push_back(res.values.release());
   export_array(static_cast<int64_t>(rows), 0, std::move(bufs), nullptr, out_array);
   return LC_OK;
 }
@@ -2004,92 +1984,24 @@ int scan_read_async(lc_ctx* ctx, FusedRead* fr, Entry* const* entries, uint64_t 
                       (proto->sh.arrow_type == BT_UTF8 || proto->sh.arrow_type == BT_BINARY);
   if ((!is_int && !is_str) || (is_int && !rl->same_width) || (is_str && !d_offsets) || !d_values || !d_header) return LC_INTERNAL_FALLBACK;
   const uint32_t tb = is_int ? proto->ih.tbits / 8 : 0;
-  cudaStream_t s = ctx->L()->stream;
-  const uint64_t cap_rows = is_int ? std::min<uint64_t>(rows_cap, values_cap / tb) : rows_cap;
-  const uint64_t cap_bytes = is_int ? 0 : std::min<uint64_t>(values_cap, 0x7fffffffull);
+  PlannedRead pr{};
+  pr.sel_base = d_sel;
+  pr.sel_off = d_word_off;
+  pr.k2 = d_counts2;
+  pr.cap_rows = is_int ? std::min<uint64_t>(rows_cap, values_cap / tb) : rows_cap;
+  pr.cap_bytes = is_int ? 0 : std::min<uint64_t>(values_cap, 0x7fffffffull);
   // dictionary-length scratch: at most min(n, cap_rows) entries have survivors, each at most the list's largest dictionary
-  const uint64_t cap_ulen = is_int ? 0 : std::min<uint64_t>(n, cap_rows) * round_up(rl->max_unique, 4);
-  uint64_t o = 0;
-  auto take = [&](uint64_t bytes) { const uint64_t at = o; o += round_up(bytes, 256); return at; };
+  pr.cap_ulen = is_int ? 0 : std::min<uint64_t>(n, pr.cap_rows) * round_up(rl->max_unique, 4);
   // A selective scan (the caller's row capacity says so: at most a handful of survivors per entry on average) is read by
-  // ONE kernel — sizes, chained scan across its CTAs, decode (k_str_read_onepass) — instead of the six launches below.
-  const bool onepass = is_str && rows_cap <= 16ull * n;
-  const uint64_t o_status = onepass ? take(((n + 7) / 8 + 2) * 8) : 0;
-  const uint64_t o_rowb = take(n * 8), o_vw = take(n * 8), o_ul = take(n * 8), o_bb = take(n * 8), o_cnt = take(n * 16);
-  const uint64_t o_rowoff = (is_str && !onepass) ? take((cap_rows + n) * 4 + 16) : 0, o_rowkey = (is_str && !onepass) ? take(cap_rows * 4 + 16) : 0;
-  const uint64_t o_ulen = (is_str && !onepass) ? take(cap_ulen * 4 + 16) : 0;
-  if (o > fr->a_cap) {
-    if (fr->a_buf) {
-      LC_CUDA_OK(cudaStreamSynchronize(s));
-      cudaFree(fr->a_buf);
-      fr->a_buf = nullptr;
-      fr->a_cap = 0;
-    }
-    if (cudaMalloc(reinterpret_cast<void**>(&fr->a_buf), o + o / 8) != cudaSuccess) {
-      cudaGetLastError();
-      return LC_INTERNAL_FALLBACK;
-    }
-    fr->a_cap = o + o / 8;
-  }
-  uint8_t* d = fr->a_buf;
-  ScanPlanHdr* d_hdr = static_cast<ScanPlanHdr*>(d_header);
-  if (onepass) {
-    StrGatherIo g{};
-    g.io.refs = rl->d_refs;
-    g.io.sel_base = d_sel;
-    g.io.sel_off = d_word_off;
-    g.k_hint = d_counts2;
-    g.out_offsets = static_cast<int32_t*>(d_offsets);
-    g.out_bytes = static_cast<uint8_t*>(d_values);
-    LC_CUDA_OK(launch_str_read_onepass(static_cast<uint32_t>(n), g, cap_rows, cap_bytes, d_hdr,
-                                       reinterpret_cast<unsigned long long*>(d + o_status), s));
-    ctx->kernel_launches++;
-    return LC_OK;
-  }
-  uint64_t* d_rowb = reinterpret_cast<uint64_t*>(d + o_rowb);
-  uint64_t* d_vw = reinterpret_cast<uint64_t*>(d + o_vw);
-  uint64_t* d_ul = reinterpret_cast<uint64_t*>(d + o_ul);
-  uint64_t* d_bb = reinterpret_cast<uint64_t*>(d + o_bb);
-  uint32_t* d_cnt = reinterpret_cast<uint32_t*>(d + o_cnt);
-  LC_CUDA_OK(cudaMemsetAsync(d_cnt, 0, n * 16, s));
-  LC_CUDA_OK(launch_scan_plan_rows(d_counts2, is_str ? rl->d_n_unique : nullptr, static_cast<uint32_t>(n), cap_rows, cap_ulen, d_rowb,
-                                   d_vw, d_ul, d_hdr, s));
-  ctx->kernel_launches++;
-  ScanIo io{};
-  io.refs = rl->d_refs;
-  io.sel_base = d_sel;
-  io.sel_off = d_word_off;
-  io.out_off = d_rowb;
-  io.valid_off = d_vw;
-  io.counts = d_cnt;
-  io.counts_stride = 4;
-  if (is_int) {
-    io.out_base = d_values;
-    io.abort_flag = &d_hdr->overflow;
-    IntPredDesc ip{};
-    LC_CUDA_OK(launch_int_scan(MODE_DECODE, static_cast<uint32_t>(n), io, ip, rl->max_blob, s));
-    ctx->kernel_launches++;
-  } else {
-    StrGatherIo g{};
-    g.io = io;
-    g.row_off_base = reinterpret_cast<uint32_t*>(d + o_rowoff);
-    g.row_key_base = reinterpret_cast<uint32_t*>(d + o_rowkey);
-    g.ulen_base = reinterpret_cast<uint32_t*>(d + o_ulen);
-    g.row_base = d_rowb;
-    g.ulen_off = d_ul;
-    g.byte_base = d_bb;
-    g.k_hint = d_counts2;
-    g.plan = d_hdr;
-    g.sparse_max = 64;
-    g.out_offsets = static_cast<int32_t*>(d_offsets);
-    g.out_bytes = static_cast<uint8_t*>(d_values);
-    LC_CUDA_OK(launch_str_lengths_sparse(static_cast<uint32_t>(n), g, s));
-    LC_CUDA_OK(launch_str_lengths(static_cast<uint32_t>(n), g, rl->max_head, s));
-    LC_CUDA_OK(launch_scan_plan_bytes(d_cnt, static_cast<uint32_t>(n), cap_bytes, d_bb, g.out_offsets, d_hdr, s));
-    LC_CUDA_OK(launch_str_decode(static_cast<uint32_t>(n), g, s));
-    ctx->kernel_launches += 4;
-  }
-  return LC_OK;
+  // ONE kernel — sizes, chained scan across its CTAs, decode (k_str_read_onepass) — instead of the general sequence.
+  pr.onepass = is_str && rows_cap <= 16ull * n;
+  const uint64_t o = planned_layout(n, is_str, pr.onepass, pr.cap_rows, pr.cap_ulen).bytes;
+  LC_TRY(grow_device(ctx->L()->stream, &fr->a_buf, &fr->a_cap, o, o / 8));
+  pr.scratch = fr->a_buf;
+  pr.d_values = d_values;
+  pr.d_offsets = is_str ? static_cast<int32_t*>(d_offsets) : nullptr;
+  pr.d_hdr = static_cast<ScanPlanHdr*>(d_header);
+  return enqueue_planned_read(ctx, rl, n, pr);
 }
 
 void fused_read_learn(FusedRead* fr, const ArrowArray* arr, int64_t value_bytes, uint64_t ulen_words) {
@@ -2110,54 +2022,43 @@ void fused_read_free(FusedRead* fr) {
 // Utf8 / Binary as is; Utf8View / BinaryView by building 16-byte views over the single data buffer;
 // Dictionary<UInt16,_> by re-encoding (what arrow's cast dictionary -> original type leaves the caller with,
 // byte_view_array/mod.rs:287-290).
-static int finish_bytes_array(const Entry* proto, uint64_t rows, uint64_t nulls, HostBuf validity, HostBuf offsets,
-                              HostBuf views, HostBuf data, ArrowSchema* out_schema, ArrowArray* out_array) {
+static int finish_bytes_array(const Entry* proto, uint64_t rows, uint64_t nulls, HostBlock validity, HostBlock offsets,
+                              HostBlock views, HostBlock data, ArrowSchema* out_schema, ArrowArray* out_array) {
   const uint8_t bt = proto->sh.arrow_type;
   const int32_t* off = reinterpret_cast<const int32_t*>(offsets.p);
   if (bt == BT_DECIMAL128 || bt == BT_DECIMAL256) {
     // LiquidFixedLenByteArray::to_arrow_array (fix_len_byte_array.rs:87-95): the decimal array itself; `views` holds the
     // values at their fixed stride (null slots zero)
-    host_free(data.p);
     export_schema(proto->arrow_format, "", out_schema);
-    std::vector<HostBuf> bufs{validity, views};
+    std::vector<HostBuf> bufs{validity.release(), views.release()};
     export_array(static_cast<int64_t>(rows), static_cast<int64_t>(nulls), std::move(bufs), nullptr, out_array);
     return LC_OK;
   }
   if (bt == BT_UTF8 || bt == BT_BINARY) {
     export_schema(bt == BT_UTF8 ? "u" : "z", "", out_schema);
-    std::vector<HostBuf> bufs{validity, offsets, data};
+    std::vector<HostBuf> bufs{validity.release(), offsets.release(), data.release()};
     export_array(static_cast<int64_t>(rows), static_cast<int64_t>(nulls), std::move(bufs), nullptr, out_array);
     return LC_OK;
   }
   if (bt == BT_UTF8_VIEW || bt == BT_BINARY_VIEW) {
     // the views came off the device (k_build_views); only the variadic-sizes buffer is made here
-    HostBuf sizes{host_alloc(8), 8};
+    HostBlock sizes(8, 8);
     if (!sizes.p) {
-      host_free(validity.p);
-      host_free(views.p);
-      host_free(data.p);
       set_error("host allocation failed");
       return LC_ERR_OOM;
     }
     const int64_t sz = static_cast<int64_t>(data.bytes);
     std::memcpy(sizes.p, &sz, 8);
     export_schema(bt == BT_UTF8_VIEW ? "vu" : "vz", "", out_schema);
-    std::vector<HostBuf> bufs{validity, views, data, sizes};
+    std::vector<HostBuf> bufs{validity.release(), views.release(), data.release(), sizes.release()};
     export_array(static_cast<int64_t>(rows), static_cast<int64_t>(nulls), std::move(bufs), nullptr, out_array);
     return LC_OK;
   }
   // Dictionary<UInt16, Utf8|Binary>: first-occurrence re-encode of the decoded rows
   std::unordered_map<std::string, uint16_t> seen;
   std::vector<std::string> order;
-  // this function owns validity / offsets / data from here on: every way out releases what the result does not keep
-  auto drop_inputs = [&]() {
-    host_free(validity.p);
-    host_free(offsets.p);
-    host_free(data.p);
-  };
-  HostBuf keys{host_alloc(rows * 2 + 2), rows * 2};
+  HostBlock keys(rows * 2 + 2, rows * 2);
   if (!keys.p) {
-    drop_inputs();
     set_error("host allocation failed");
     return LC_ERR_OOM;
   }
@@ -2170,8 +2071,6 @@ static int finish_bytes_array(const Entry* proto, uint64_t rows, uint64_t nulls,
     uint16_t key;
     if (it == seen.end()) {
       if (order.size() >= 65536) {
-        host_free(keys.p);
-        drop_inputs();
         set_error("more than 65536 distinct values in a dictionary result");
         return LC_ERR_UNSUPPORTED_TYPE;
       }
@@ -2185,13 +2084,9 @@ static int finish_bytes_array(const Entry* proto, uint64_t rows, uint64_t nulls,
   }
   uint64_t dbytes = 0;
   for (auto& sv : order) dbytes += sv.size();
-  HostBuf doff{host_alloc((order.size() + 1) * 4), (order.size() + 1) * 4};
-  HostBuf ddata{host_alloc(dbytes ? dbytes : 1), dbytes};
+  HostBlock doff((order.size() + 1) * 4, (order.size() + 1) * 4);
+  HostBlock ddata(dbytes ? dbytes : 1, dbytes);
   if (!doff.p || !ddata.p) {
-    host_free(doff.p);
-    host_free(ddata.p);
-    host_free(keys.p);
-    drop_inputs();
     set_error("host allocation failed");
     return LC_ERR_OOM;
   }
@@ -2203,13 +2098,11 @@ static int finish_bytes_array(const Entry* proto, uint64_t rows, uint64_t nulls,
     p += order[i].size();
   }
   dof[order.size()] = static_cast<int32_t>(p);
-  host_free(offsets.p);
-  host_free(data.p);
   ArrowArray dict_arr;
-  std::vector<HostBuf> dbufs{HostBuf{nullptr, 0}, doff, ddata};
+  std::vector<HostBuf> dbufs{HostBuf{nullptr, 0}, doff.release(), ddata.release()};
   export_array(static_cast<int64_t>(order.size()), 0, std::move(dbufs), nullptr, &dict_arr);
   export_schema("S", bt == BT_DICT16_UTF8 ? "u" : "z", out_schema);
-  std::vector<HostBuf> bufs{validity, keys};
+  std::vector<HostBuf> bufs{validity.release(), keys.release()};
   export_array(static_cast<int64_t>(rows), static_cast<int64_t>(nulls), std::move(bufs), &dict_arr, out_array);
   return LC_OK;
 }

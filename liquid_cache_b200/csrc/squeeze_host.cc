@@ -629,32 +629,22 @@ int squeezed_component_array(lc_ctx* ctx, Entry* sq, int32_t lossy, ArrowSchema*
   LC_CUDA_OK(launch_date_lossy(reinterpret_cast<const int32_t*>(comp.p), nulls ? reinterpret_cast<const uint32_t*>(val.p) : nullptr, n,
                                sq->date_field, ticks, res.p, s));
   ctx->kernel_launches++;
-  HostBuf values{host_alloc(static_cast<uint64_t>(n) * out_tb), static_cast<uint64_t>(n) * out_tb};
-  HostBuf validity;
+  HostBlock values(static_cast<uint64_t>(n) * out_tb, static_cast<uint64_t>(n) * out_tb);
+  HostBlock validity;
   if (nulls) {
-    validity.bytes = (static_cast<uint64_t>(n) + 7) / 8;
-    validity.p = host_alloc(round_up(validity.bytes, 4));
+    const uint64_t bitmap_bytes = (static_cast<uint64_t>(n) + 7) / 8;
+    validity = HostBlock(round_up(bitmap_bytes, 4), bitmap_bytes);
   }
   if ((n && !values.p) || (nulls && !validity.p)) {
-    host_free(values.p);
-    host_free(validity.p);
     set_error("host allocation failed");
     return LC_ERR_OOM;
   }
-  cudaError_t ce = n ? cudaMemcpyAsync(values.p, res.p, static_cast<uint64_t>(n) * out_tb, cudaMemcpyDeviceToHost, s) : cudaSuccess;
-  if (ce == cudaSuccess && nulls) ce = cudaMemcpyAsync(validity.p, val.p, round_up(validity.bytes, 4), cudaMemcpyDeviceToHost, s);
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-  if (ce != cudaSuccess) {
-    host_free(values.p);
-    host_free(validity.p);
-    set_error("CUDA error in lc_squeezed_component: %s", cudaGetErrorString(ce));
-    return LC_ERR_CUDA;
-  }
+  if (n) LC_CUDA_OK(cudaMemcpyAsync(values.p, res.p, static_cast<uint64_t>(n) * out_tb, cudaMemcpyDeviceToHost, s));
+  if (nulls) LC_CUDA_OK(cudaMemcpyAsync(validity.p, val.p, round_up(validity.bytes, 4), cudaMemcpyDeviceToHost, s));
+  LC_CUDA_OK(cudaStreamSynchronize(s));
   ctx->d2h_bytes += values.bytes + validity.bytes;
   export_schema(sq->orig_format, "", out_schema);
-  std::vector<HostBuf> bufs;
-  bufs.push_back(validity);
-  bufs.push_back(values);
+  std::vector<HostBuf> bufs{validity.release(), values.release()};
   export_array(static_cast<int64_t>(n), static_cast<int64_t>(nulls), std::move(bufs), nullptr, out_array);
   return LC_OK;
 }
